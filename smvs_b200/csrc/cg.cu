@@ -55,7 +55,6 @@
  * of a CTA then stream separate pieces of H instead of one contiguous piece).
  */
 #include <algorithm>
-#include <cstdlib>
 #include <cstring>
 
 #include "common.cuh"
@@ -93,8 +92,7 @@ struct CgView
     double* Ad;
     double* z;
     double* partials;        /* [CG_SLOTS][CG_MAX_BLOCKS] */
-    double* result;          /* [0] iterations, [1] info, [2] isnan(x[0]),
-                                [4..7] phase times in ns (timing build) */
+    double* result;          /* [0] iterations, [1] info, [2] isnan(x[0]) */
 };
 
 struct CgArgs
@@ -141,17 +139,6 @@ grid_barrier (unsigned int* counter, unsigned int& epoch)
             : "=r"(v) : "l"(counter) : "memory");
     }
     __syncthreads();
-}
-
-template <bool TIMING>
-__device__ __forceinline__ unsigned long long
-now_ns (void)
-{
-    if (!TIMING)
-        return 0;
-    unsigned long long t;
-    asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
-    return t;
 }
 
 /* L2 evict-first access policy. Not volatile: the compiler may hoist it out
@@ -415,7 +402,7 @@ pass_row (CgView const& V, int n_rows, int pass, int& node)
  * values fetched per pass. The kernel is bound by the number of loads a warp
  * has in flight, and every dependent fetch in front of a pass's Hessian loads
  * lengthens the time a warp spends per pass. */
-template <bool TIMING, int NV>
+template <int NV>
 __global__ void __launch_bounds__(CG_THREADS, 2)
 cg_kernel (CgArgs const a)
 {
@@ -506,7 +493,6 @@ cg_kernel (CgArgs const a)
     __syncthreads();
 
     int iter = 1;
-    unsigned long long tm[4] = {0, 0, 0, 0};
     /* The rows and masks do not change during a solve: the first pass's of
      * every view are fetched once. */
     int first_node[NV];
@@ -528,17 +514,12 @@ cg_kernel (CgArgs const a)
     }
     for (; iter < a.max_iter; ++iter)
     {
-        unsigned long long const t_a = now_ns<TIMING>();
         /* the direction is double buffered; all views swap in lock-step */
         bool const odd = (iter & 1) != 0;
         int const slot = 2 + 4 * (iter & 1);
 
         /* d = z + beta d_old (:192-198 of the previous iteration);
-         * Ad = A d; alpha = r_dot_r / d.Ad (:126-127). Software pipeline over
-         * the passes: the row index travels two passes ahead of the stream,
-         * its mask one pass ahead, and the first two rows of the NEXT view are
-         * fetched while this view streams, so no load of a pass waits for
-         * another one. */
+         * Ad = A d; alpha = r_dot_r / d.Ad (:126-127). */
         {
             /* One pass = the CTA's 64 block rows; the next pass's row index
              * and mask are fetched while this pass streams. (A deeper
@@ -583,9 +564,7 @@ cg_kernel (CgArgs const a)
             }
             publish<1>(a, s_state, s_red, slot, false);
         }
-        unsigned long long const t_b = now_ns<TIMING>();
         grid_barrier(a.sync, epoch);
-        unsigned long long const t_c = now_ns<TIMING>();
         all_sums<1>(a, s_state, slot, s_bcast, false);
         if (threadIdx.x < a.n_views && !s_state[threadIdx.x].done)
             s_state[threadIdx.x].alpha = s_state[threadIdx.x].r_dot_r
@@ -669,14 +648,8 @@ cg_kernel (CgArgs const a)
             warp_flush<3>(acc, s_red, v);
         }
         publish<3>(a, s_state, s_red, slot + 1, false);
-        unsigned long long const t_d = now_ns<TIMING>();
         grid_barrier(a.sync, epoch);
         all_sums<3>(a, s_state, slot + 1, s_bcast, false);
-        if (TIMING)
-        {
-            tm[0] += t_b - t_a; tm[1] += t_c - t_b;
-            tm[2] += t_d - t_c; tm[3] += now_ns<TIMING>() - t_d;
-        }
 
         /* the reference's two stopping tests, per view (:139, :170-176) */
         if (threadIdx.x < a.n_views && !s_state[threadIdx.x].done)
@@ -725,8 +698,6 @@ cg_kernel (CgArgs const a)
         /* lib/depth_optimizer.cc:267 looks at the first entry of the solution;
          * the final barrier has made every CTA's x visible */
         res[2] = isnan(__ldcg(a.v[threadIdx.x].x)) ? 1.0 : 0.0;
-        for (int i = 0; i < 4; ++i)
-            res[4 + i] = static_cast<double>(tm[i]);
     }
 }
 
@@ -902,20 +873,15 @@ cg_enqueue (smvsb_ctx* const* cs, int n, int max_iter, double err_tol,
     if (n < 1 || n > SMVSB_MAX_BATCH)
         throw Error(SMVSB_ERR_INVALID, "batch size out of range");
     smvsb_ctx* lead = cs[0];
-    bool const timing = getenv("SMVSB_CG_TIMING") != nullptr;
     void const* kernel = nullptr;
     if (n == 1)
-        kernel = timing ? (void const*)cg_kernel<true, 1>
-            : (void const*)cg_kernel<false, 1>;
+        kernel = (void const*)cg_kernel<1>;
     else if (n == 2)
-        kernel = timing ? (void const*)cg_kernel<true, 2>
-            : (void const*)cg_kernel<false, 2>;
+        kernel = (void const*)cg_kernel<2>;
     else if (n <= 4)
-        kernel = timing ? (void const*)cg_kernel<true, 4>
-            : (void const*)cg_kernel<false, 4>;
+        kernel = (void const*)cg_kernel<4>;
     else
-        kernel = timing ? (void const*)cg_kernel<true, 8>
-            : (void const*)cg_kernel<false, 8>;
+        kernel = (void const*)cg_kernel<8>;
 
     int per_sm = 0;
     CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm,
@@ -966,9 +932,8 @@ cg_enqueue (smvsb_ctx* const* cs, int n, int max_iter, double err_tol,
     for (int k = 0; k < n; ++k)
     {
         smvsb_ctx* c = cs[k];
-        c->cg_grid = grid;
         CUDA_CHECK(cudaMemcpyAsync(c->h_scalars, c->cg_result.p,
-            8 * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+            3 * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
         CUDA_CHECK(cudaMemcpyAsync(c->h_scalars + 8, c->cg_counts.p,
             2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost,
             c->stream));
@@ -981,11 +946,6 @@ cg_collect (smvsb_ctx* c, int* iters, int* info, bool* x0_nan)
     double const* res = c->h_scalars;
     unsigned long long counts[2];
     std::memcpy(counts, c->h_scalars + 8, sizeof(counts));
-    if (getenv("SMVSB_CG_TIMING"))
-        fprintf(stderr, "cg: iters %d grid %d | us/iter: spmv %.1f wait %.1f | "
-            "update %.1f wait %.1f\n", (int)res[0], c->cg_grid,
-            res[4] / 1e3 / res[0], res[5] / 1e3 / res[0], res[6] / 1e3 / res[0],
-            res[7] / 1e3 / res[0]);
     c->cg_blocks = counts[0];
     c->cg_rows = counts[1];
     if (iters) *iters = static_cast<int>(res[0]);

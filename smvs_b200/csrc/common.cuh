@@ -168,7 +168,6 @@ struct smvsb_ctx
     smvsb::DevBuf<uint32_t> cg_row_list, cg_block_rows;
     smvsb::DevBuf<unsigned long long> cg_counts;
     uint64_t cg_blocks = 0, cg_rows = 0;    /* of the last solve's system */
-    int cg_grid = 0;
     double* h_scalars = nullptr;        /* pinned, 32 doubles: results of the
                                            asynchronous read-backs */
     smvsb::DevBuf<unsigned int> cg_sync;

@@ -1,39 +1,32 @@
 /*
  * sgm.cu -- SGMStereo::run_sgm on the GPU (reference: lib/sgm_stereo.cc).
  *
- *   K6  sgm_cost_kernel     create_cost_volume (:192-244): plane sweep of the
- *                           neighbour luminance at num_steps inverse-depth
- *                           planes (warped_neighbors_for_depth :150-190, fp32,
- *                           byte bilinear with +0.5 rounding), 9x7 census
- *                           (:126-148) of main image and of every warped
- *                           slice, Hamming distance; 255 where the warped
- *                           pixel is 0. The reference materialises the warped
- *                           volume (uint8) and its census volume (uint64,
- *                           2.1 GB at 2 MP x 128); here a block keeps the
- *                           warped tile (with halo) of four planes in shared
- *                           memory, compares two pixels per integer add
- *                           (16-bit fields) and only the uint8 cost leaves
- *                           the SM.
- *   K7  sgm_paths_kernel    aggregate_sgm_costs (:429-667), SSE branch
- *                           (constant P2, uint16 arithmetic): one warp per
- *                           scan line of a direction, all 8 directions in one
- *                           launch; disparities across the lanes, L_r carried
- *                           in registers, min over disparities by warp
- *                           shuffles. Diagonals follow the line with
- *                           wrap-around at the image border, where the
- *                           reference restarts the path (:515-534). Each
- *                           direction writes L_r - C (a byte) to its own volume.
- *   K8  sgm_sum_wta_kernel  S = 8 C + sum_r (L_r - C) (+ the reference's
- *                           corner extras) and depth_from_sgm_volume
- *                           (:274-306) in one pass; S is only materialised
- *                           when the caller asks for the volume.
+ *   K6  create_cost_volume (:192-244): u8_to_float_kernel (float copy of the
+ *       neighbour image), sgm_warp_volume_kernel (plane sweep of the
+ *       neighbour luminance at num_steps inverse-depth planes,
+ *       warped_neighbors_for_depth :150-190: fp32, byte bilinear with +0.5
+ *       rounding, into a uint8 volume), sgm_cost_bits_kernel (9x7 census
+ *       :126-148 of the main image and of every warped slice, Hamming
+ *       distance; 255 where the warped pixel is 0). The census words never
+ *       leave the SM (the reference's uint64 census volume is 2.1 GB at
+ *       2 MP x 128).
+ *   K7  aggregate_sgm_costs (:429-667), SSE branch (constant P2, uint16
+ *       arithmetic): sgm_paths128_kernel at 128 planes, sgm_paths_kernel<DPL>
+ *       otherwise. All 8 directions in one launch, warps on scan lines,
+ *       disparities across the lanes, L_r carried in registers, min over
+ *       disparities by warp shuffles. Diagonals wrap around at the image
+ *       border, where the reference restarts the path (:515-534). Each
+ *       direction writes L_r - C (a byte) to its own volume.
+ *   K8  S = 8 C + sum_r (L_r - C) (+ the reference's corner extras) and
+ *       depth_from_sgm_volume (:274-306) in one pass: sgm_sum_wta128_kernel
+ *       at 128 planes, sgm_sum_wta_kernel<DPL> otherwise; S is only
+ *       materialised when the caller asks for the volume.
  *
  * Layouts: cost C[pixel][disp] uint8, sum S[pixel][disp] uint16 (pixel-major,
  * disparity contiguous, like the reference's sse_*_volume), so a warp's
  * access to one pixel is one coalesced 128 B / 256 B segment.
  */
 #include <algorithm>
-#include <cstdlib>
 #include <mutex>
 
 #include <cuda_fp16.h>
@@ -52,40 +45,19 @@ struct SgmParams
 };
 
 /*
- * Cost volume. A thread owns two horizontally adjacent pixels and works on
- * four depth planes at a time.
- *
- *  - The 63 census comparisons per pixel run on the half-precision pipe, two
- *    pixels per instruction: pixels (0..255, exact in fp16) are kept as
- *    half2 pairs; for centre pair A and neighbour pair B, HSET2.LT gives
- *    c = (A < B) as 1.0 / 0.0 per half.
- *  - The Hamming distance of two census words does not depend on the bit
- *    order, so no 63-bit word is ever assembled, and it is linear in the
- *    warped slice's bits once the main image's bits are known:
- *        distance = sum_o [c_w(o) != c_m(o)] = K + sum_o s(o) c_w(o),
- *    s(o) = +1 where c_m(o) = 0, -1 where it is 1, K = popcount(c_m). The
- *    signs of a block's main pixels are computed once into shared memory
- *    (63 KB) and reused for all planes; per offset and plane a pixel pair
- *    costs one HSET2 and one HFMA2 (|sum| <= 63 is exact in fp16) -- on the
- *    FMA pipe, which the integer formulation (three ALU-pipe instructions)
- *    left idle.
- *  - The warped slice of a 32 x 16 pixel tile with its 9x7 halo is computed
- *    once per plane into shared memory by the whole block (fp32 steps
- *    restated with explicit round-to-nearest ops, so bit-identical to the
- *    CPU); M * (x, y, 1) does not depend on the plane and is kept in
- *    registers. Integer <-> float conversions run on the quarter-rate XU
- *    pipe: the neighbour image is read from a float copy, floor() is taken
- *    with the 1.5 * 2^23 trick.
+ * Cost volume, in three launches: the neighbour image as floats, the warped
+ * volume (sgm_warp_volume_kernel), then census + Hamming distance
+ * (sgm_cost_bits_kernel), four depth planes per iteration.
+ *  - The warp restates the reference's fp32 steps with explicit
+ *    round-to-nearest ops, so it is bit-identical to the CPU; M * (x, y, 1)
+ *    does not depend on the plane and is kept in registers. Integer <-> float
+ *    conversions run on the quarter-rate XU pipe: the neighbour image is read
+ *    from a float copy, floor() is taken with the 1.5 * 2^23 trick.
  * Semantics restated from census_filter / create_cost_volume
  * (lib/sgm_stereo.cc:126-148, 192-244): census only for pixels with
  * 4 <= x < w-5, 3 <= y < h-4 and a non-zero centre; cost 255 where the
  * warped pixel is 0.
  */
-constexpr int CT_W = 32, CT_H = 16;              /* pixel tile per block */
-constexpr int CT_THREADS = (CT_W / 2) * CT_H;    /* 256: one pixel pair each */
-constexpr int HALO_W = CT_W + 8, HALO_H = CT_H + 6;
-constexpr int HALO_N = HALO_W * HALO_H;          /* 880 */
-constexpr int HALO_PER_THREAD = (HALO_N + CT_THREADS - 1) / CT_THREADS;
 constexpr int PLANES = 4;                        /* planes per iteration */
 
 /* floor of 0 <= x < 2^22 as a float and as an int, without F2I / I2F */
@@ -106,7 +78,6 @@ floor_pos (float x, float& fl, int& n)
 /* warped_neighbors_for_depth (lib/sgm_stereo.cc:150-190) for one pixel and
  * plane: the neighbour's luminance as the byte value the reference stores
  * (0 = no sample). neigh: float copy of the byte image. */
-template <bool F2I>
 __device__ __forceinline__ unsigned
 warp_from_tp (SgmParams const& p, float const* __restrict__ neigh,
     float const* tp, float depth, float nw1, float nh1)
@@ -144,20 +115,10 @@ warp_from_tp (SgmParams const& p, float const* __restrict__ neigh,
     s = __fadd_rn(s, __fmul_rn(v11, __fmul_rn(w1, w3)));
     s = __fadd_rn(s, 0.5f);
     /* static_cast<uint8_t>(s): truncation, 0 <= s < 256. One conversion
-     * instruction on the otherwise idle XU pipe, or six on the ALU / FMA
-     * pipes the kernel is bound by (A/B: SMVSB_SGM_NO_F2I=1) */
-    if (F2I)
-        return __float2uint_rz(s);
-    float fl;
-    int n;
-    floor_pos(s, fl, n);
-    return static_cast<unsigned>(n);
+     * instruction on the otherwise idle XU pipe instead of six on the
+     * ALU / FMA pipes the kernel is bound by */
+    return __float2uint_rz(s);
 }
-
-/* Pair of 16-bit fields at element offset e (0..8) of the five words
- * wd[0..4] that hold elements 0..9 of a tile row. */
-#define SMVSB_WINDOW(wd, e) (((e) & 1) ? __funnelshift_r((wd)[(e) >> 1],   \
-    (wd)[((e) >> 1) + 1], 16) : (wd)[(e) >> 1])
 
 __device__ __forceinline__ __half2
 as_half2 (unsigned v)
@@ -188,13 +149,12 @@ u8_to_float_kernel (size_t n, uint8_t const* __restrict__ in,
  * (4 columns, 3 rows, rounded up to the cost kernel's tiles) is part of the
  * volume, so the cost kernel loads its tiles without bounds tests. One thread
  * warps four neighbouring pixels through all planes (M * (x, y, 1) stays in
- * registers) and stores one word per plane; every voxel is warped ONCE (inside
- * the cost kernel the tiles' halos overlap and every voxel was warped 1.7
- * times, two thirds of that kernel's instructions).
+ * registers) and stores one word per plane; every voxel is warped ONCE
+ * (warping inside the cost kernel would repeat it wherever the tiles' halos
+ * overlap, 1.7 times per voxel).
  */
 constexpr int WV_BX = 32, WV_BY = 4;
 
-template <bool F2I>
 __global__ void __launch_bounds__(WV_BX * WV_BY)
 sgm_warp_volume_kernel (SgmParams const p, float const* __restrict__ neigh,
     float const* __restrict__ depths, uint8_t* __restrict__ Wv, int pitch,
@@ -250,7 +210,7 @@ sgm_warp_volume_kernel (SgmParams const p, float const* __restrict__ neigh,
         {
             unsigned v = 0;
             if (in_img[k])
-                v = warp_from_tp<F2I>(p, neigh, tp[k], depth, nw1, nh1);
+                v = warp_from_tp(p, neigh, tp[k], depth, nw1, nh1);
             word |= v << (8 * k);
         }
         dst[d * (plane_stride / 4)] = word;
@@ -260,147 +220,7 @@ sgm_warp_volume_kernel (SgmParams const p, float const* __restrict__ neigh,
 /*
  * Census + Hamming distance from the warped volume. Pixels enter the fp16
  * comparisons as 1024 + byte (0x6400 | byte: one PRMT turns two bytes into a
- * half2, no conversion instruction; the order of the values is the bytes').
- */
-__global__ void __launch_bounds__(CT_THREADS, 2)
-sgm_cost_kernel (SgmParams const p, uint8_t const* __restrict__ main_img,
-    uint8_t const* __restrict__ Wv, int pitch, int rows,
-    uint8_t* __restrict__ cost)
-{
-    /* tile of fp16 pixels, HALO_W even; as words: HALO_W / 2 per row */
-    __shared__ unsigned s_tile[PLANES][HALO_H][HALO_W / 2];
-    /* signs of the main comparison bits, [63][CT_THREADS] half2 = 63 KB:
-     * dynamic */
-    extern __shared__ unsigned s_mask_dyn[];
-    unsigned (*s_mask)[CT_THREADS] =
-        reinterpret_cast<unsigned (*)[CT_THREADS]>(s_mask_dyn);
-
-    int const tid = threadIdx.x;
-    int const tx = tid % (CT_W / 2), ty = tid / (CT_W / 2);
-    int const x0 = blockIdx.x * CT_W, y0 = blockIdx.y * CT_H;
-    int const px = x0 + 2 * tx, py = y0 + ty;        /* left pixel of the pair */
-
-    /* main image tile -> signs of its comparison bits per offset */
-    __half* tile16 = reinterpret_cast<__half*>(&s_tile[0][0][0]);
-#pragma unroll
-    for (int k = 0; k < HALO_PER_THREAD; ++k)
-    {
-        int const i = tid + k * CT_THREADS;
-        if (i < HALO_N)
-        {
-            int const gx = x0 - 4 + i % HALO_W, gy = y0 - 3 + i / HALO_W;
-            bool const in = (gx >= 0 && gx < p.w && gy >= 0 && gy < p.h);
-            tile16[i] = __ushort2half_rn(in ? main_img[gy * p.w + gx] : 0);
-        }
-    }
-    __syncthreads();
-    bool const in0 = (px < p.w && py < p.h), in1 = (px + 1 < p.w && py < p.h);
-    bool const int0 = in0 && px >= 4 && px < p.w - 5 && py >= 3 && py < p.h - 4;
-    bool const int1 = in1 && px + 1 >= 4 && px + 1 < p.w - 5 && py >= 3
-        && py < p.h - 4;
-    __half2 K2 = __float2half2_rn(0.0f);
-    {
-        __half2 const A = as_half2(s_tile[0][ty + 3][tx + 2]);
-        /* pixels without a census (border, zero centre): all bits 0 */
-        __half2 const keep = __floats2half2_rn(
-            (int0 && __low2float(A) != 0.0f) ? 1.0f : 0.0f,
-            (int1 && __high2float(A) != 0.0f) ? 1.0f : 0.0f);
-        __half2 const one = __float2half2_rn(1.0f);
-        __half2 const mtwo = __float2half2_rn(-2.0f);
-#pragma unroll
-        for (int j = 0; j < 7; ++j)
-        {
-            unsigned wd[5];
-#pragma unroll
-            for (int q = 0; q < 5; ++q) wd[q] = s_tile[0][ty + j][tx + q];
-#pragma unroll
-            for (int e = 0; e < 9; ++e)
-            {
-                __half2 const B = as_half2(SMVSB_WINDOW(wd, e));
-                __half2 const cm = __hmul2(__hlt2(A, B), keep);
-                K2 = __hadd2(K2, cm);
-                s_mask[j * 9 + e][tid] = as_word(__hfma2(cm, mtwo, one));
-            }
-        }
-    }
-
-    size_t const plane_stride = static_cast<size_t>(pitch) * rows;
-    constexpr int ROW_WORDS = HALO_W / 4;                    /* 10 */
-    constexpr int TILE_WORDS = PLANES * HALO_H * ROW_WORDS;  /* 880 */
-    for (int d0 = 0; d0 < p.D; d0 += PLANES)
-    {
-        __syncthreads();
-        /* the four planes' tiles: aligned words of four bytes -> two half2 */
-        for (int i = tid; i < TILE_WORDS; i += CT_THREADS)
-        {
-            int const pl = i / (HALO_H * ROW_WORDS);
-            int const rem = i % (HALO_H * ROW_WORDS);
-            int const r = rem / ROW_WORDS, q = rem % ROW_WORDS;
-            unsigned const b = __ldg(reinterpret_cast<unsigned const*>(Wv
-                + (d0 + pl) * plane_stride
-                + static_cast<size_t>(y0 + r) * pitch + x0) + q);
-            *reinterpret_cast<uint2*>(&s_tile[pl][r][2 * q]) = make_uint2(
-                __byte_perm(b, 0x64646464u, 0x4140),
-                __byte_perm(b, 0x64646464u, 0x4342));
-        }
-        __syncthreads();
-
-        __half2 A[PLANES], acc[PLANES];
-#pragma unroll
-        for (int pl = 0; pl < PLANES; ++pl)
-        {
-            A[pl] = as_half2(s_tile[pl][ty + 3][tx + 2]);
-            acc[pl] = K2;
-        }
-#pragma unroll
-        for (int j = 0; j < 7; ++j)
-        {
-            unsigned wd[PLANES][5];
-#pragma unroll
-            for (int pl = 0; pl < PLANES; ++pl)
-#pragma unroll
-                for (int q = 0; q < 5; ++q)
-                    wd[pl][q] = s_tile[pl][ty + j][tx + q];
-#pragma unroll
-            for (int e = 0; e < 9; ++e)
-            {
-                __half2 const sg = as_half2(s_mask[j * 9 + e][tid]);
-#pragma unroll
-                for (int pl = 0; pl < PLANES; ++pl)
-                {
-                    __half2 const B = as_half2(SMVSB_WINDOW(wd[pl], e));
-                    acc[pl] = __hfma2(__hlt2(A[pl], B), sg, acc[pl]);
-                }
-            }
-        }
-        /* cost bytes of the four planes for each of the two pixels */
-        unsigned out0 = 0, out1 = 0;
-#pragma unroll
-        for (int pl = 0; pl < PLANES; ++pl)
-        {
-            /* border pixels have no census on either side: distance 0 */
-            unsigned c0 = int0 ? static_cast<unsigned>(
-                __half2int_rn(__low2half(acc[pl]))) : 0u;
-            unsigned c1 = int1 ? static_cast<unsigned>(
-                __half2int_rn(__high2half(acc[pl]))) : 0u;
-            /* warped pixel 0 (= 1024 here): no sample */
-            if ((as_word(A[pl]) & 0xffffu) == 0x6400u) c0 = 255u;
-            if ((as_word(A[pl]) & 0xffff0000u) == 0x64000000u) c1 = 255u;
-            out0 |= c0 << (8 * pl);
-            out1 |= c1 << (8 * pl);
-        }
-        if (in0)
-            *reinterpret_cast<unsigned*>(cost + (static_cast<size_t>(py) * p.w
-                + px) * p.D + d0) = out0;
-        if (in1)
-            *reinterpret_cast<unsigned*>(cost + (static_cast<size_t>(py) * p.w
-                + px + 1) * p.D + d0) = out1;
-    }
-}
-
-/*
- * Census + Hamming distance, second formulation (round 2): comparison BITS
- * instead of signed sums, collected on the FMA pipe. A thread owns four
+ * half2; the order of the values is the bytes'). A thread owns four
  * neighbouring pixels (two half2 pairs); per offset and plane a pair costs
  * one HSET2 (1.0 where centre < neighbour) and one HFMA2 that adds
  * 2^e to the accumulator of the window row: an accumulator starts at 1024.0
@@ -409,13 +229,12 @@ sgm_cost_kernel (SgmParams const p, uint8_t const* __restrict__ main_img,
  * conversion. The main image's bits are built the same way once per block
  * and stay in fourteen REGISTERS; distance = popcount of the XOR (two rows
  * per POPC after a byte permute).
- * Why: the signed-sum kernel read 63 sign words per pair and iteration from
- * shared memory and was bound by the shared-memory queue (ncu: mio throttle
- * stalls); collecting the bits with HSET2 mask
- * output + LOP3 moved everything onto the half-rate ALU pipe. Here the per-offset work is split between the ALU pipe (HSET2)
- * and the FMA pipe (HFMA2), and the odd-offset windows come from a second
- * copy of the tile shifted by one pixel (an LDS instead of a funnel shift).
- * Tiles are 64 x 16 pixels (halo redundancy 1.55 instead of 1.72), loaded as
+ * Why bits: a signed-sum formulation reads 63 sign words per pair and
+ * iteration from shared memory and is bound by the shared-memory queue.
+ * The per-offset work is split between the ALU pipe (HSET2) and the FMA
+ * pipe (HFMA2), and the odd-offset windows come from a second copy of the
+ * tile shifted by one pixel (an LDS instead of a funnel shift). Tiles are
+ * 64 x 16 pixels (halo redundancy 1.55; 1.72 at 32 x 16), loaded as
  * aligned words one iteration ahead into the other half of a double buffer.
  */
 constexpr int C2_W = 64, C2_H = 16;
@@ -647,7 +466,6 @@ sgm_cost_bits_kernel (SgmParams const p, uint8_t const* __restrict__ main_img,
     }
 }
 #undef SMVSB_ROW_BITS
-#undef SMVSB_WINDOW
 
 /* ------------------------------------------------------------------ */
 
@@ -667,15 +485,19 @@ enum PathKind
  * and copy_cost_and_add_to_sgm (:408-426) where a path starts (L = C).
  * The directions cannot share one read-modify-write sum volume without
  * racing, so each writes its own byte volume of L - C, which lies in [0, P2]
- * (P2 <= 255): 1 B/voxel/direction. sgm_sum_wta_kernel adds them up.
+ * (P2 <= 255): 1 B/voxel/direction. The sum / WTA kernels add them up.
  */
 /*
  * 128 planes, TWO scan lines per warp: a half-warp owns a line, a lane eight
- * disparities (four registers of 16-bit pairs). The kernel is bound by
+ * disparities (four registers of 16-bit pairs; the minima are DPX
+ * instructions, and L <= C + P2 <= 510 never overflows a half, so packed
+ * adds / subtracts are plain 32-bit ones). The kernel is bound by
  * instruction issue, and the per-step bookkeeping (position, pointers, the
  * shuffle tree of min_k, the loop) costs the same for 256 voxels as it does
- * for 128 in the one-line-per-warp kernel below; the tree is one level
- * shorter. The two lines of a warp are neighbours of the same direction, so
+ * for 128 with one line per warp; the tree is one level shorter too. A step
+ * moves both pointers by a constant (plus or minus one image row where a
+ * diagonal wraps around), and the next step's costs are fetched one step
+ * ahead. The two lines of a warp are neighbours of the same direction, so
  * they take the same number of steps; a diagonal restarts at different steps
  * on the two, hence no branch around the shuffles: the recurrence is always
  * evaluated and a restarting line overrides it.
@@ -839,91 +661,9 @@ sgm_paths_kernel (int w, int h, unsigned P1, unsigned P2,
 
     auto load_cost = [&](size_t base, unsigned* C)
     {
-        if (DPL == 4)
-        {
-            uchar4 const c4 = *reinterpret_cast<uchar4 const*>(cost + base);
-            C[0] = c4.x; C[1] = c4.y; C[2] = c4.z; C[3] = c4.w;
-        }
-        else
-        {
 #pragma unroll
-            for (int i = 0; i < DPL; ++i) C[i] = cost[base + i];
-        }
+        for (int i = 0; i < DPL; ++i) C[i] = cost[base + i];
     };
-
-    if (DPL == 4)
-    {
-        /* Fast path for 128 planes: the four disparities of a lane live in
-         * two registers as 16-bit pairs; the minima are DPX instructions
-         * (VIMNMX3 / VIADDMNMX on 16x2). L <= C + P2 <= 510 never overflows a
-         * half, so packed adds / subtracts are plain 32-bit ones. */
-        unsigned const P1x2 = P1 | (P1 << 16), P2x2 = P2 | (P2 << 16);
-        unsigned const BIG = 0x7000u;      /* "no neighbour" sentinel */
-        unsigned P01 = 0, P23 = 0;
-        /* The kernel is bound by instruction issue (ncu: issue slots 77 %
-         * busy, DRAM 25 %), so the per-step bookkeeping is kept to pointer
-         * increments: a step moves both pointers by a constant, a diagonal
-         * that leaves the image at one side re-enters at the other (where the
-         * reference restarts the path, :515-534) with a correction of one
-         * image row. The cost word of the next step is fetched one step ahead
-         * (two or four ahead cost more instructions than they hide). */
-        long long const row_bytes = static_cast<long long>(w) * D;
-        long long const step_bytes = dy * row_bytes + dx * D;
-        uint8_t const* pc = cost + (static_cast<size_t>(y) * w + x) * D
-            + lane * 4;
-        uint8_t* pd = Dr + (static_cast<size_t>(y) * w + x) * D + lane * 4;
-        unsigned c4 = *reinterpret_cast<unsigned const*>(pc);
-        bool start = true;
-        for (int s = 0; s < steps; ++s)
-        {
-            /* next position */
-            int xn = x + dx;
-            long long adv = step_bytes;
-            if (xn < 0) { xn = w - 1; adv += row_bytes; }
-            if (xn >= w) { xn = 0; adv -= row_bytes; }
-            unsigned c4n = 0;
-            if (s + 1 < steps)
-                c4n = *reinterpret_cast<unsigned const*>(pc + adv);
-
-            unsigned const C01 = __byte_perm(c4, 0, 0x4140);
-            unsigned const C23 = __byte_perm(c4, 0, 0x4342);
-            unsigned D01 = 0, D23 = 0;
-            if (start)
-            {
-                P01 = C01; P23 = C23;
-            }
-            else
-            {
-                unsigned const m2 = __vminu2(P01, P23);
-                unsigned mn = min(m2 & 0xffffu, m2 >> 16);
-                for (int off = 16; off > 0; off >>= 1)
-                    mn = min(mn, __shfl_xor_sync(0xffffffffu, mn, off));
-                unsigned below = __shfl_up_sync(0xffffffffu, P23, 1) >> 16;
-                unsigned above = __shfl_down_sync(0xffffffffu, P01, 1)
-                    & 0xffffu;
-                if (lane == 0) below = BIG;
-                if (lane == 31) above = BIG;
-                unsigned const mid = (P01 >> 16) | (P23 << 16);   /* L1, L2 */
-                unsigned const lo01 = below | (P01 << 16);        /* -, L0 */
-                unsigned const hi23 = (P23 >> 16) | (above << 16);/* L3, - */
-                unsigned const mn2 = mn * 0x10001u;
-                unsigned const far2 = mn2 + P2x2;
-                unsigned const b01 = __vimin3_u16x2(P01, far2,
-                    __viaddmin_u16x2(mid, P1x2, lo01 + P1x2));
-                unsigned const b23 = __vimin3_u16x2(P23, far2,
-                    __viaddmin_u16x2(hi23, P1x2, mid + P1x2));
-                D01 = b01 - mn2;          /* = L - C, in [0, P2] per half */
-                D23 = b23 - mn2;
-                P01 = C01 + D01;
-                P23 = C23 + D23;
-            }
-            *reinterpret_cast<unsigned*>(pd) = __byte_perm(D01, D23, 0x6420);
-            c4 = c4n;
-            x = xn; pc += adv; pd += adv;
-            start = diagonal && (xn == restart_x);
-        }
-        return;
-    }
 
     unsigned Lp[DPL], C[DPL];
 #pragma unroll
@@ -978,16 +718,9 @@ sgm_paths_kernel (int w, int h, unsigned P1, unsigned P2,
 #pragma unroll
             for (int i = 0; i < DPL; ++i) Lp[i] = Ln[i];
         }
-        if (DPL == 4)
-            *reinterpret_cast<uchar4*>(Dr + base) = make_uchar4(
-                (unsigned char)Dv[0], (unsigned char)Dv[1],
-                (unsigned char)Dv[2], (unsigned char)Dv[3]);
-        else
-        {
 #pragma unroll
-            for (int i = 0; i < DPL; ++i)
-                Dr[base + i] = static_cast<uint8_t>(Dv[i]);
-        }
+        for (int i = 0; i < DPL; ++i)
+            Dr[base + i] = static_cast<uint8_t>(Dv[i]);
 #pragma unroll
         for (int i = 0; i < DPL; ++i) C[i] = Cn[i];
         x = xn; y = yn; base = basen; start = startn;
@@ -1067,7 +800,7 @@ sgm_sum_wta_kernel (int w, int h, uint8_t const* __restrict__ cost,
  * fields (S < 9 * 255 + 8 * 255: no carry between the fields), and the
  * argmin -- lowest value, then lowest index, like the reference's first
  * minimum -- runs over the lane's 16 values and then over the pixel's eight
- * lanes. The byte-load version spent its time in the load/store unit
+ * lanes. With byte loads the kernel spends its time in the load/store unit
  * (lg_throttle and mio_throttle stalls).
  */
 __device__ __forceinline__ void
@@ -1163,18 +896,19 @@ void
 run_paths (int w, int h, unsigned P1, unsigned P2, uint8_t const* cost,
     uint8_t* Dvol, cudaStream_t st)
 {
-    if (DPL == 4 && getenv("SMVSB_SGM_PATHS_1LINE") == nullptr)
+    if constexpr (DPL == 4)
     {
         /* two lines per warp */
         int const warps = 2 * ((h + 1) / 2) + 6 * ((w + 1) / 2);
         sgm_paths128_kernel<<<(warps * 32 + 127) / 128, 128, 0, st>>>(w, h,
             P1, P2, cost, Dvol);
-        CUDA_CHECK(cudaGetLastError());
-        return;
     }
-    int const warps = 2 * h + 6 * w;
-    sgm_paths_kernel<DPL><<<(warps * 32 + 127) / 128, 128, 0, st>>>(w, h, P1,
-        P2, cost, Dvol);
+    else
+    {
+        int const warps = 2 * h + 6 * w;
+        sgm_paths_kernel<DPL><<<(warps * 32 + 127) / 128, 128, 0, st>>>(w, h,
+            P1, P2, cost, Dvol);
+    }
     CUDA_CHECK(cudaGetLastError());
 }
 
@@ -1184,17 +918,18 @@ run_wta (int w, int h, uint8_t const* cost, uint8_t const* Dvol,
     uint8_t const* main_img, float const* depths, uint16_t* S_out, float* out,
     cudaStream_t st)
 {
-    if (DPL == 4 && getenv("SMVSB_SGM_WTA_BYTES") == nullptr)
+    if constexpr (DPL == 4)
     {
         int const blocks8 = (w * h * 8 + 255) / 256;
         sgm_sum_wta128_kernel<<<blocks8, 256, 0, st>>>(w, h, cost, Dvol,
             main_img, depths, S_out, out);
-        CUDA_CHECK(cudaGetLastError());
-        return;
     }
-    int const blocks = (w * h * 32 + 255) / 256;
-    sgm_sum_wta_kernel<DPL><<<blocks, 256, 0, st>>>(w, h, cost, Dvol, main_img,
-        depths, S_out, out);
+    else
+    {
+        int const blocks = (w * h * 32 + 255) / 256;
+        sgm_sum_wta_kernel<DPL><<<blocks, 256, 0, st>>>(w, h, cost, Dvol,
+            main_img, depths, S_out, out);
+    }
     CUDA_CHECK(cudaGetLastError());
 }
 
@@ -1385,43 +1120,22 @@ sgm_pair (SgmWorkspace& ws, int w, int h, uint8_t const* main_dev, int nw,
     CUDA_CHECK(cudaGetLastError());
     /* warped volume with the cost tiles' halo as margin (zeros, written by
      * the kernel itself) */
-    bool const bits = getenv("SMVSB_SGM_COST_SUMS") == nullptr;
-    int const tile_w = bits ? C2_W : CT_W;
-    int const pitch = (w + tile_w - 1) / tile_w * tile_w + 16;
-    int const rows = (h + CT_H - 1) / CT_H * CT_H + 6;
+    int const pitch = (w + C2_W - 1) / C2_W * C2_W + 16;
+    int const rows = (h + C2_H - 1) / C2_H * C2_H + 6;
     ws.d_warp.reserve(static_cast<size_t>(pitch) * rows * num_steps);
     dim3 const wb(WV_BX, WV_BY);
     dim3 const wg((pitch / 4 + WV_BX - 1) / WV_BX, (rows + WV_BY - 1) / WV_BY);
-    if (getenv("SMVSB_SGM_NO_F2I") == nullptr)
-        sgm_warp_volume_kernel<true><<<wg, wb, 0, st>>>(p, ws.d_neigh_f.p,
-            depths_dev, ws.d_warp.p, pitch, rows);
-    else
-        sgm_warp_volume_kernel<false><<<wg, wb, 0, st>>>(p, ws.d_neigh_f.p,
-            depths_dev, ws.d_warp.p, pitch, rows);
+    sgm_warp_volume_kernel<<<wg, wb, 0, st>>>(p, ws.d_neigh_f.p, depths_dev,
+        ws.d_warp.p, pitch, rows);
     CUDA_CHECK(cudaGetLastError());
-    if (bits)
-    {
-        dim3 const cg((w + C2_W - 1) / C2_W, (h + C2_H - 1) / C2_H);
-        size_t const tile_bytes = sizeof(unsigned) * 2 * 2 * PLANES
-            * C2_HALO_H * C2_ROW_WORDS;
-        CUDA_CHECK(cudaFuncSetAttribute(sgm_cost_bits_kernel,
-            cudaFuncAttributeMaxDynamicSharedMemorySize,
-            static_cast<int>(tile_bytes)));
-        sgm_cost_bits_kernel<<<cg, C2_THREADS, tile_bytes, st>>>(p, main_dev,
-            ws.d_warp.p, pitch, rows, ws.d_cost.p);
-    }
-    else
-    {
-        /* the signed-sum formulation (A/B: SMVSB_SGM_COST_SUMS=1) */
-        dim3 const cb(CT_THREADS);
-        dim3 const cg((w + CT_W - 1) / CT_W, (h + CT_H - 1) / CT_H);
-        size_t const mask_bytes = 63 * CT_THREADS * sizeof(unsigned);
-        CUDA_CHECK(cudaFuncSetAttribute(sgm_cost_kernel,
-            cudaFuncAttributeMaxDynamicSharedMemorySize,
-            static_cast<int>(mask_bytes)));
-        sgm_cost_kernel<<<cg, cb, mask_bytes, st>>>(p, main_dev, ws.d_warp.p,
-            pitch, rows, ws.d_cost.p);
-    }
+    dim3 const cg((w + C2_W - 1) / C2_W, (h + C2_H - 1) / C2_H);
+    size_t const tile_bytes = sizeof(unsigned) * 2 * 2 * PLANES
+        * C2_HALO_H * C2_ROW_WORDS;
+    CUDA_CHECK(cudaFuncSetAttribute(sgm_cost_bits_kernel,
+        cudaFuncAttributeMaxDynamicSharedMemorySize,
+        static_cast<int>(tile_bytes)));
+    sgm_cost_bits_kernel<<<cg, C2_THREADS, tile_bytes, st>>>(p, main_dev,
+        ws.d_warp.p, pitch, rows, ws.d_cost.p);
     CUDA_CHECK(cudaGetLastError());
     CUDA_CHECK(cudaEventRecord(ws.ev[e0 + 1], st));
 

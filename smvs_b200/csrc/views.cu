@@ -430,15 +430,13 @@ set_scale_tma_kernel (T const* __restrict__ img, int w, int h, int R,
 }
 
 /* Launches the fused kernel if the image qualifies; false = use the three
- * kernels (pitch not a multiple of 16 bytes, very large blur radius, or
- * SMVSB_NO_TMA set -- the A/B switch of benchmarks/set_scale_bench.py). */
+ * kernels (pitch not a multiple of 16 bytes, misaligned image, or a blur
+ * radius too large for shared memory). */
 template <typename T>
 bool
 try_set_scale_tma (smvsb_ctx* c, T const* img_dev, int w, int h,
     BlurKernel const& k, int mode, float* out_dev, float* blur_out)
 {
-    if (getenv("SMVSB_NO_TMA") != nullptr)
-        return false;
     if ((static_cast<size_t>(w) * sizeof(T)) % 16 != 0
         || reinterpret_cast<uintptr_t>(img_dev) % 16 != 0)
         return false;

@@ -343,7 +343,8 @@ def test_live_full_opt_mean_shift():
 
 
 @needs_ref
-@pytest.mark.parametrize("w,h,D", [(333, 207, 64), (640, 480, 128), (200, 150, 32)])
+@pytest.mark.parametrize("w,h,D", [(333, 207, 64), (640, 480, 128), (200, 150, 32),
+                                   (200, 150, 256)])
 def test_live_sgm_bit_exact(w, h, D):
     sc = synth.make_scene(w, h, 1, seed_index=9)
     R = oref.RefScene(sc)
