@@ -27,6 +27,18 @@
  * lib/gauss_newton_step.cc:91-105), so a system that has shrunk to 10 % of
  * the grid costs 10 % of the vector traffic as well.
  *
+ * H does not change during a solve, and a CTA's first pass (its 64 block
+ * rows) is the same in every iteration: for a single view the kernel copies
+ * those rows into shared memory once per solve (TMA bulk copies at kernel
+ * start, waited for before the first SpMV) and reads them from there. With
+ * 2 CTAs on each of the H100's 132 SMs that is 16 896 rows held on chip: the
+ * full system (119 064 rows at 1920x1080 scale 2) streams 14 % less of H per
+ * iteration, and the systems of the last Newton steps of a loop, which fit
+ * in one pass, stream none after the copy. (Shared memory, unlike the L2
+ * pinning below, takes no space from the vectors; it comes out of L1, 73 KB
+ * per CTA.) Where each value of H is read from is all that changes: the
+ * arithmetic, and so the result, is bitwise the same.
+ *
  * Several views per launch (smvsb_newton_loop_batch; the reference runs one
  * view per pool thread, app/smvsrecon.cc:658-733): what an iteration costs
  * besides the Hessian stream is two grid-wide synchronisations, a fixed
@@ -329,16 +341,56 @@ struct DirVec
     }
 };
 
+/*
+ * Where spmv_row reads a block row of H from. StreamRows: the matrix in HBM,
+ * streamed. PinnedRows: the copy of the CTA's pass-0 rows in shared memory
+ * (one row per quad, CG_PIN_STRIDE doubles apart), see cg_kernel.
+ */
+struct StreamRows
+{
+    double const* H;
+    __device__ __forceinline__ double const* row (int node, int rp) const
+    {
+        return H + static_cast<size_t>(node) * 144 + rp * 4;
+    }
+    __device__ __forceinline__ void load (double const* p, double2& h01,
+        double2& h23) const
+    {
+        ld_stream(p, h01, h23);
+    }
+};
+
+/* Row stride 146 doubles (1168 B) rather than 144: with 1152 B the eight
+ * quads of a warp hit the same 16 banks and every LDS.128 takes 8 wavefronts;
+ * 1168 B moves odd quads onto the other 16 banks, the ideal 4. */
+constexpr int CG_PIN_STRIDE = 146;
+constexpr size_t CG_PIN_BYTES = sizeof(double) * CG_PIN_STRIDE * CG_QUADS;
+
+struct PinnedRows
+{
+    double const* s;
+    __device__ __forceinline__ double const* row (int, int rp) const
+    {
+        return s + (threadIdx.x >> 2) * CG_PIN_STRIDE + rp * 4;
+    }
+    __device__ __forceinline__ void load (double const* p, double2& h01,
+        double2& h23) const
+    {
+        h01 = *reinterpret_cast<double2 const*>(p);
+        h23 = *reinterpret_cast<double2 const*>(p + 2);
+    }
+};
+
 /* (H v)[node, rp] for the thread's node and block row, blocks visited in
  * the reference's order (ascending column block,
  * lib/block_sparse_matrix.h:283-296). own[] receives v[node]. */
-template <typename VecOp>
+template <typename Rows, typename VecOp>
 __device__ __forceinline__ double
-spmv_row (double const* __restrict__ H, int ns, VecOp const& vec, int node,
-    int rp, unsigned int mask, double* own)
+spmv_row (Rows const& H, int ns, VecOp const& vec, int node, int rp,
+    unsigned int mask, double* own)
 {
     int const ix = node % ns, iy = node / ns;
-    double const* hrow = H + static_cast<size_t>(node) * 144 + rp * 4;
+    double const* hrow = H.row(node, rp);
     double acc = 0.0;
     own[0] = 0.0; own[1] = 0.0; own[2] = 0.0; own[3] = 0.0;
     /* The reference drops the rows and columns of inactive nodes
@@ -357,7 +409,7 @@ spmv_row (double const* __restrict__ H, int ns, VecOp const& vec, int node,
         int const jx = ix + (k % 3) - 1, jy = iy + (k / 3) - 1;
         int const nj = jy * ns + jx;
         double2 h01, h23;
-        ld_stream(hrow + k * 16, h01, h23);
+        H.load(hrow + k * 16, h01, h23);
         double v[4];
         vec.load(nj, v);
         if (k == 4)
@@ -417,9 +469,15 @@ cg_kernel (CgArgs const a)
      * once registers are tight -- ncu: short-scoreboard stalls 4.0 instead of
      * 0.7 per issue, SpMV phase +20 %.) */
     __shared__ double const* s_zptr[NV];
+    /* NV = 1: the H rows of the CTA's pass 0 (CG_PIN_BYTES, dynamic) and the
+     * mbarrier their copies complete on */
+    extern __shared__ __align__(16) double s_pin[];
+    __shared__ __align__(8) unsigned long long s_pin_bar;
     unsigned int epoch = 0;
     int const quad = threadIdx.x & 28;      /* first lane of the node's quad */
     int const rp = threadIdx.x & 3;
+    unsigned const pin_bar = static_cast<unsigned>(
+        __cvta_generic_to_shared(&s_pin_bar));
 
     if (threadIdx.x < a.n_views)
     {
@@ -434,8 +492,46 @@ cg_kernel (CgArgs const a)
         S.partials = V.partials;
         S.grid = V.grid;
         s_zptr[threadIdx.x] = V.z;
+        if (NV == 1)
+        {
+            int const n_pin = static_cast<int>(blockIdx.x) < V.grid
+                ? min(max(S.n_rows - static_cast<int>(blockIdx.x) * CG_QUADS,
+                  0), CG_QUADS) : 0;
+            if (n_pin > 0)
+            {
+                asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;"
+                    :: "r"(pin_bar), "r"(n_pin));
+                asm volatile("fence.mbarrier_init.release.cluster;"
+                    ::: "memory");
+            }
+        }
     }
     __syncthreads();
+
+    /* H does not change during the solve: the block rows of the CTA's pass 0
+     * are copied into shared memory once, by the TMA engine (one 1152-byte
+     * bulk copy per row, issued by the row's first thread), and the SpMV
+     * reads them from there in every iteration. The copies travel while the
+     * initialisation phase runs; the mbarrier counts one arrival per row
+     * plus its bytes. */
+    bool const pin = NV == 1 && static_cast<int>(blockIdx.x) < s_state[0].grid
+        && static_cast<int>(blockIdx.x) * CG_QUADS < s_state[0].n_rows;
+    if (NV == 1 && rp == 0)
+    {
+        int node;
+        if (static_cast<int>(blockIdx.x) < s_state[0].grid
+            && pass_row(a.v[0], s_state[0].n_rows, 0, node))
+        {
+            unsigned const dst = static_cast<unsigned>(__cvta_generic_to_shared(
+                s_pin + (threadIdx.x >> 2) * CG_PIN_STRIDE));
+            double const* src = a.v[0].H + static_cast<size_t>(node) * 144;
+            asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], "
+                "%1;" :: "r"(pin_bar), "r"(1152) : "memory");
+            asm volatile("cp.async.bulk.shared::cluster.global"
+                ".mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                :: "r"(dst), "l"(src), "r"(1152), "r"(pin_bar) : "memory");
+        }
+    }
 
     /* r = b = -g; x = 0 (host memset); z = P r; r_dot_r = z.r; ||g||^2
      * (lib/conjugate_gradient.h:85-117). d_old = 0 with beta = 0 makes the
@@ -512,6 +608,15 @@ cg_kernel (CgArgs const a)
             }
         }
     }
+    if (pin)
+    {
+        unsigned done = 0;
+        while (!done)
+            asm volatile("{\n.reg .pred p;\n"
+                "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], 0;\n"
+                "selp.u32 %0, 1, 0, p;\n}"
+                : "=r"(done) : "r"(pin_bar) : "memory");
+    }
     for (; iter < a.max_iter; ++iter)
     {
         /* the direction is double buffered; all views swap in lock-step */
@@ -541,7 +646,7 @@ cg_kernel (CgArgs const a)
                 double acc[1] = { 0.0 };
                 int node = first_node[v];
                 unsigned int mask = first_mask[v];
-                for (int q = quad0; q < n_rows; q += quads)
+                auto row_pass = [&](auto const& rows, int q)
                 {
                     int const qn = q + quads;
                     int const node_next = (qn < n_rows)
@@ -550,7 +655,7 @@ cg_kernel (CgArgs const a)
                         ? V.rowmask[node_next] : 0u;
                     double own[4];
                     size_t const i = static_cast<size_t>(node) * 4 + rp;
-                    double const val = spmv_row(V.H, V.npx + 1, dir, node, rp,
+                    double const val = spmv_row(rows, V.npx + 1, dir, node, rp,
                         mask, own);
                     node = node_next;
                     mask = mask_next;
@@ -559,7 +664,15 @@ cg_kernel (CgArgs const a)
                     V.Ad[i] = val;
                     d_new[i] = di;
                     acc[0] += val * di;
+                };
+                int q = quad0;
+                if (NV == 1 && q < n_rows)
+                {
+                    row_pass(PinnedRows{ s_pin }, q);
+                    q += quads;
                 }
+                for (; q < n_rows; q += quads)
+                    row_pass(StreamRows{ V.H }, q);
                 warp_flush<1>(acc, s_red, v);
             }
             publish<1>(a, s_state, s_red, slot, false);
@@ -819,8 +932,9 @@ spmv_kernel (int n_nodes, int npx, double const* __restrict__ H,
         return;
     PlainVec vec;
     vec.v = x;
+    StreamRows const rows{ H };
     double own[4];
-    y[i] = spmv_row(H, npx + 1, vec, i >> 2, i & 3, rowmask[i >> 2], own);
+    y[i] = spmv_row(rows, npx + 1, vec, i >> 2, i & 3, rowmask[i >> 2], own);
 }
 
 /* The system's row masks, counts and compacted row list (three small kernels
@@ -883,11 +997,38 @@ cg_enqueue (smvsb_ctx* const* cs, int n, int max_iter, double err_tol,
     else
         kernel = (void const*)cg_kernel<8>;
 
+    /* cg_kernel<1> keeps its pass-0 rows of H in shared memory: ask for a
+     * carveout that holds two CTAs and leaves the rest of the SM's 256 KB to
+     * L1 */
+    size_t const dyn_smem = (n == 1) ? CG_PIN_BYTES : 0;
+    if (n == 1)
+    {
+        cudaFuncAttributes fa;
+        CUDA_CHECK(cudaFuncGetAttributes(&fa, kernel));
+        int smem_sm = 0, reserved = 0;
+        CUDA_CHECK(cudaDeviceGetAttribute(&smem_sm,
+            cudaDevAttrMaxSharedMemoryPerMultiprocessor, lead->device));
+        CUDA_CHECK(cudaDeviceGetAttribute(&reserved,
+            cudaDevAttrReservedSharedMemoryPerBlock, lead->device));
+        size_t const need = 2 * (dyn_smem + fa.sharedSizeBytes + reserved);
+        int const carveout = static_cast<int>(std::min<size_t>(100,
+            (100 * need + smem_sm - 1) / smem_sm));
+        CUDA_CHECK(cudaFuncSetAttribute(kernel,
+            cudaFuncAttributeMaxDynamicSharedMemorySize,
+            static_cast<int>(dyn_smem)));
+        CUDA_CHECK(cudaFuncSetAttribute(kernel,
+            cudaFuncAttributePreferredSharedMemoryCarveout, carveout));
+    }
     int per_sm = 0;
     CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm,
-        kernel, CG_THREADS, 0));
+        kernel, CG_THREADS, dyn_smem));
     if (per_sm < 1)
         throw Error(SMVSB_ERR_CUDA, "cg_kernel does not fit on an SM");
+    /* the grid size fixes the order of the grid-wide sums: a single view is
+     * solved with 2 CTAs/SM or not at all */
+    if (n == 1 && per_sm < 2)
+        throw Error(SMVSB_ERR_CUDA, "cg_kernel<1> fits only "
+            + std::to_string(per_sm) + " CTA per SM, needs 2");
     /* (Two views in flight on one GPU with 1 CTA/SM each, so that one view's
      * SpMV runs under the other's barriers and vector update, was slower end
      * to end than 2 CTAs/SM with the two launches taking turns.) */
@@ -926,7 +1067,7 @@ cg_enqueue (smvsb_ctx* const* cs, int n, int max_iter, double err_tol,
     CUDA_CHECK(cudaMemsetAsync(a.sync, 0, sizeof(unsigned int), lead->stream));
     void* params[] = { &a };
     CUDA_CHECK(cudaLaunchCooperativeKernel(kernel, dim3(grid),
-        dim3(CG_THREADS), params, 0, lead->stream));
+        dim3(CG_THREADS), params, dyn_smem, lead->stream));
     smvsb::count_launches(lead, 1);
     CUDA_CHECK(cudaGetLastError());
     for (int k = 0; k < n; ++k)
