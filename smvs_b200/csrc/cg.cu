@@ -81,6 +81,8 @@ constexpr int CG_QUADS = CG_THREADS / 4;     /* block rows per CTA and pass */
 constexpr int CG_MAX_BLOCKS = 1024;
 constexpr int CG_UF = 4;          /* rows per thread in flight, update phase */
 constexpr int CG_SLOTS = 10;      /* partial-sum slots per view */
+constexpr int CG_ROW_CACHE = 16;  /* row-list passes per CTA held in shared
+                                     memory, shared out among the NV views */
 
 /* One view's system and vectors. */
 struct CgView
@@ -261,13 +263,13 @@ publish (CgArgs const& a, CgState const* s_state, double const* s_red,
 /* Every CTA sums, per view, the partials of slots first .. first+NV-1 of all
  * the view's CTAs in the same order: one warp per (view, slot), lane l adds
  * partials l, l+32, ... in sequence (loads issued in batches ahead of the
- * adds), then the shuffle tree. Results in s_bcast[view * 3 + j]. */
+ * adds), then the shuffle tree. Results in s_bcast[view * 3 + j]. Called
+ * right after grid_barrier, whose closing bar.sync orders it. */
 template <int NV>
 __device__ __forceinline__ void
 all_sums (CgArgs const& a, CgState const* s_state, int first_slot,
     double* s_bcast, bool init)
 {
-    __syncthreads();
     int const warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     for (int pair = warp; pair < a.n_views * NV; pair += CG_WARPS)
     {
@@ -445,6 +447,71 @@ pass_row (CgView const& V, int n_rows, int pass, int& node)
     return ok;
 }
 
+/* The row list does not change during a solve: the nodes and masks of the
+ * first PASSES passes of every view (per quad of the CTA; node 0 and mask 0
+ * past the end of the list) are loaded into shared memory once, so that a
+ * phase does not begin with the dependent rows[] -> rowmask[] fetches through
+ * L2 (the grid barrier's acquire has just emptied L1). */
+template <int NV>
+struct RowCache
+{
+    static constexpr int PASSES = CG_ROW_CACHE / NV;
+    uint32_t node[NV][PASSES][CG_QUADS];
+    uint16_t mask[NV][PASSES][CG_QUADS];
+};
+
+template <int NV>
+__device__ __forceinline__ void
+fill_rows (RowCache<NV>& c, CgArgs const& a, CgState const* s_state)
+{
+    constexpr int N = RowCache<NV>::PASSES * CG_QUADS;
+#pragma unroll
+    for (int v = 0; v < NV; ++v)
+    {
+#pragma unroll
+        for (int k = 0; k < (N + CG_THREADS - 1) / CG_THREADS; ++k)
+        {
+            int const e = k * CG_THREADS + threadIdx.x;
+            if (e >= N)
+                break;
+            int const p = e / CG_QUADS, qd = e % CG_QUADS;
+            int node = 0;
+            unsigned int mask = 0u;
+            if (v < a.n_views && static_cast<int>(blockIdx.x) < s_state[v].grid)
+            {
+                int const q = p * (s_state[v].grid * CG_QUADS)
+                    + blockIdx.x * CG_QUADS + qd;
+                if (q < s_state[v].n_rows)
+                {
+                    node = static_cast<int>(a.v[v].rows[q]);
+                    mask = a.v[v].rowmask[node];
+                }
+            }
+            c.node[v][p][qd] = static_cast<uint32_t>(node);
+            c.mask[v][p][qd] = static_cast<uint16_t>(mask);
+        }
+    }
+}
+
+/* pass_row, and the row's mask: from the cache for the first passes. */
+template <int NV>
+__device__ __forceinline__ bool
+cached_row (RowCache<NV> const& c, CgView const& V, int v, int n_rows,
+    int pass, int& node, unsigned int& mask)
+{
+    if (pass < RowCache<NV>::PASSES)
+    {
+        int const qd = threadIdx.x >> 2;
+        node = static_cast<int>(c.node[v][pass][qd]);
+        mask = c.mask[v][pass][qd];
+        return pass * (V.grid * CG_QUADS) + static_cast<int>(blockIdx.x)
+            * CG_QUADS + qd < n_rows;
+    }
+    bool const ok = pass_row(V, n_rows, pass, node);
+    mask = ok ? V.rowmask[node] : 0u;
+    return ok;
+}
+
 /* 2 CTAs / SM: measured faster than 3 at 80 registers (fewer loads hoisted,
  * more barrier participants).
  *
@@ -473,6 +540,7 @@ cg_kernel (CgArgs const a)
      * mbarrier their copies complete on */
     extern __shared__ __align__(16) double s_pin[];
     __shared__ __align__(8) unsigned long long s_pin_bar;
+    __shared__ RowCache<NV> s_rows;
     unsigned int epoch = 0;
     int const quad = threadIdx.x & 28;      /* first lane of the node's quad */
     int const rp = threadIdx.x & 3;
@@ -532,6 +600,8 @@ cg_kernel (CgArgs const a)
                 :: "r"(dst), "l"(src), "r"(1152), "r"(pin_bar) : "memory");
         }
     }
+    /* read from the first SpMV on, behind the initialisation's barriers */
+    fill_rows(s_rows, a, s_state);
 
     /* r = b = -g; x = 0 (host memset); z = P r; r_dot_r = z.r; ||g||^2
      * (lib/conjugate_gradient.h:85-117). d_old = 0 with beta = 0 makes the
@@ -589,25 +659,6 @@ cg_kernel (CgArgs const a)
     __syncthreads();
 
     int iter = 1;
-    /* The rows and masks do not change during a solve: the first pass's of
-     * every view are fetched once. */
-    int first_node[NV];
-    unsigned int first_mask[NV];
-#pragma unroll
-    for (int v = 0; v < NV; ++v)
-    {
-        first_node[v] = 0;
-        first_mask[v] = 0u;
-        if (v < a.n_views && static_cast<int>(blockIdx.x) < s_state[v].grid)
-        {
-            int const quad0 = blockIdx.x * CG_QUADS + (threadIdx.x >> 2);
-            if (quad0 < s_state[v].n_rows)
-            {
-                first_node[v] = static_cast<int>(a.v[v].rows[quad0]);
-                first_mask[v] = a.v[v].rowmask[first_node[v]];
-            }
-        }
-    }
     if (pin)
     {
         unsigned done = 0;
@@ -627,8 +678,9 @@ cg_kernel (CgArgs const a)
          * Ad = A d; alpha = r_dot_r / d.Ad (:126-127). */
         {
             /* One pass = the CTA's 64 block rows; the next pass's row index
-             * and mask are fetched while this pass streams. (A deeper
-             * pipeline -- index two passes ahead, mask one -- was slower.) */
+             * and mask are fetched while this pass streams (from s_rows, or
+             * past its passes from the row list). (A deeper pipeline -- index
+             * two passes ahead, mask one -- was slower.) */
 #pragma unroll
             for (int v = 0; v < NV; ++v)
             {
@@ -644,15 +696,15 @@ cg_kernel (CgArgs const a)
                 dir.beta = s_state[v].beta;
                 double* d_new = odd ? V.d2 : V.d;
                 double acc[1] = { 0.0 };
-                int node = first_node[v];
-                unsigned int mask = first_mask[v];
-                auto row_pass = [&](auto const& rows, int q)
+                int node;
+                unsigned int mask;
+                cached_row(s_rows, V, v, n_rows, 0, node, mask);
+                auto row_pass = [&](auto const& rows, int p)
                 {
-                    int const qn = q + quads;
-                    int const node_next = (qn < n_rows)
-                        ? static_cast<int>(V.rows[qn]) : 0;
-                    unsigned int const mask_next = (qn < n_rows)
-                        ? V.rowmask[node_next] : 0u;
+                    int node_next;
+                    unsigned int mask_next;
+                    cached_row(s_rows, V, v, n_rows, p + 1, node_next,
+                        mask_next);
                     double own[4];
                     size_t const i = static_cast<size_t>(node) * 4 + rp;
                     double const val = spmv_row(rows, V.npx + 1, dir, node, rp,
@@ -665,14 +717,15 @@ cg_kernel (CgArgs const a)
                     d_new[i] = di;
                     acc[0] += val * di;
                 };
-                int q = quad0;
+                int q = quad0, p = 0;
                 if (NV == 1 && q < n_rows)
                 {
-                    row_pass(PinnedRows{ s_pin }, q);
+                    row_pass(PinnedRows{ s_pin }, p);
                     q += quads;
+                    ++p;
                 }
-                for (; q < n_rows; q += quads)
-                    row_pass(StreamRows{ V.H }, q);
+                for (; q < n_rows; q += quads, ++p)
+                    row_pass(StreamRows{ V.H }, p);
                 warp_flush<1>(acc, s_red, v);
             }
             publish<1>(a, s_state, s_red, slot, false);
@@ -699,9 +752,10 @@ cg_kernel (CgArgs const a)
             double acc[3] = { 0.0, 0.0, 0.0 };    /* r.r, x.(r - g), z.r */
             int nodes[CG_UF];
             bool oks[CG_UF];
+            unsigned int unused;
 #pragma unroll
             for (int u = 0; u < CG_UF; ++u)
-                oks[u] = pass_row(V, n_rows, u, nodes[u]);
+                oks[u] = cached_row(s_rows, V, v, n_rows, u, nodes[u], unused);
             /* CG_UF rows per thread in flight: the pass is latency bound */
             for (int p = 0; p < passes; p += CG_UF)
             {
@@ -709,8 +763,8 @@ cg_kernel (CgArgs const a)
                 bool oks_next[CG_UF];
 #pragma unroll
                 for (int u = 0; u < CG_UF; ++u)
-                    oks_next[u] = pass_row(V, n_rows, p + CG_UF + u,
-                        nodes_next[u]);
+                    oks_next[u] = cached_row(s_rows, V, v, n_rows,
+                        p + CG_UF + u, nodes_next[u], unused);
 
                 double xv[CG_UF], rv[CG_UF], gv[CG_UF];
                 double2 p01[CG_UF], p23[CG_UF];
