@@ -86,13 +86,17 @@ class RefScene:
     def set_scale(self, scale):
         self.L.ref_scene_set_scale(self.h_, int(scale))
 
+    def shape(self, v):
+        """(height, width) of view v; neighbours may differ from the main view."""
+        return self.scene.images[v].shape[:2]
+
     def gradients(self, v):
-        out = np.empty((self.h, self.w, 2), dtype=np.float32)
+        out = np.empty(self.shape(v) + (2,), dtype=np.float32)
         self.L.ref_view_get_gradients(self.h_, v, _p(out))
         return out
 
     def hessian(self, v):
-        out = np.empty((self.h, self.w, 3), dtype=np.float32)
+        out = np.empty(self.shape(v) + (3,), dtype=np.float32)
         self.L.ref_view_get_hessian(self.h_, v, _p(out))
         return out
 
@@ -100,7 +104,7 @@ class RefScene:
         """StereoView::get_scaleimage(): the blurred image with all its channels."""
         im = self.scene.images[v]
         ch = 1 if im.ndim == 2 else im.shape[2]
-        out = np.empty((self.h, self.w, ch), dtype=np.float32)
+        out = np.empty(self.shape(v) + (ch,), dtype=np.float32)
         self.L.ref_view_get_scaleimage(self.h_, v, _p(out))
         return out[:, :, 0] if ch == 1 else out
 

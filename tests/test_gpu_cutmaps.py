@@ -23,19 +23,21 @@ def surface_grad(x, y):
             -0.3 * 0.9 * np.sin(1.1 * x) * np.sin(0.9 * y))
 
 
-def make_views(n, w, h, seed, normal_sign=-1.0):
+def make_views(n, w, h, seed, normal_sign=-1.0, sizes=None):
     """n pinhole views of the height field z = surface(x, y): cameras near the
     plane z = 0 looking along +z with small rotations. Depth maps in MVE
     convention (distance along the ray), normal maps in world space, facing
     the cameras (normal_sign = -1; +1 gives back-facing normals, which the cut
     removes altogether); a few
     regions are pushed off the surface or removed so that every branch of the
-    cut runs."""
+    cut runs. sizes: per-view (w, h, flen) in place of w x h at flen 1.1."""
     rng = np.random.default_rng(seed)
-    flen = np.full(n, 1.1, np.float32)
+    sizes = sizes or [(w, h, 1.1)] * n
+    flen = np.array([f for _, _, f in sizes], np.float32)
     rots, transs, depths, normals = [], [], [], []
-    ys, xs = np.mgrid[0:h, 0:w]
     for k in range(n):
+        w, h = sizes[k][:2]
+        ys, xs = np.mgrid[0:h, 0:w]
         ang = rng.uniform(-0.06, 0.06, size=3)
         cx, cy, cz = np.cos(ang), np.sin(ang), None
         Rx = np.array([[1, 0, 0], [0, cx[0], -cy[0]], [0, cy[0], cx[0]]])
