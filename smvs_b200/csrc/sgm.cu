@@ -11,16 +11,16 @@
  *       leave the SM (the reference's uint64 census volume is 2.1 GB at
  *       2 MP x 128).
  *   K7  aggregate_sgm_costs (:429-667), SSE branch (constant P2, uint16
- *       arithmetic): sgm_paths128_kernel at 128 planes, sgm_paths_kernel<DPL>
- *       otherwise. All 8 directions in one launch, warps on scan lines,
- *       disparities across the lanes, L_r carried in registers, min over
- *       disparities by warp shuffles. Diagonals wrap around at the image
+ *       arithmetic): sgm_paths_kernel<L>, L = D / 8 lanes per scan line.
+ *       All 8 directions in one launch, warps on scan lines, disparities
+ *       across the lanes, L_r carried in registers, min over disparities by
+ *       warp shuffles. Diagonals wrap around at the image
  *       border, where the reference restarts the path (:515-534). Each
  *       direction writes L_r - C (a byte) to its own volume.
  *   K8  S = 8 C + sum_r (L_r - C) (+ the reference's corner extras) and
- *       depth_from_sgm_volume (:274-306) in one pass: sgm_sum_wta128_kernel
- *       at 128 planes, sgm_sum_wta_kernel<DPL> otherwise; S is only
- *       materialised when the caller asks for the volume.
+ *       depth_from_sgm_volume (:274-306) in one pass: sgm_sum_wta_kernel<G>,
+ *       G = D / 16 lanes per pixel; S is only materialised when the caller
+ *       asks for the volume.
  *
  * Layouts: cost C[pixel][disp] uint8, sum S[pixel][disp] uint16 (pixel-major,
  * disparity contiguous, like the reference's sse_*_volume), so a warp's
@@ -475,60 +475,68 @@ enum PathKind
     PATH_B2T, PATH_B2T_D1, PATH_B2T_D2
 };
 
+__host__ __device__ constexpr int
+ilog2 (int n)
+{
+    return n > 1 ? 1 + ilog2(n / 2) : 0;
+}
+
 /*
- * All eight path directions in ONE launch: warp -> (direction, scan line),
- * 2h + 6w warps in flight (13 680 at 1920x1080) instead of h or w per
- * sequential launch. DPL = disparities per lane (D = 32 * DPL).
+ * All eight path directions in ONE launch: warp -> (direction, scan lines),
+ * 2h + 6w scan lines in flight (13 680 at 1920x1080) instead of h or w per
+ * sequential launch.
  * fill_path_cost_sse (:361-406):
  *   L(p,i) = C(p,i) + min(L(q,i), L(q,i-1)+P1, L(q,i+1)+P1, min_k L(q,k)+P2)
  *            - min_k L(q,k)            (all uint16, wrap-around)
  * and copy_cost_and_add_to_sgm (:408-426) where a path starts (L = C).
  * The directions cannot share one read-modify-write sum volume without
  * racing, so each writes its own byte volume of L - C, which lies in [0, P2]
- * (P2 <= 255): 1 B/voxel/direction. The sum / WTA kernels add them up.
- */
-/*
- * 128 planes, TWO scan lines per warp: a half-warp owns a line, a lane eight
- * disparities (four registers of 16-bit pairs; the minima are DPX
- * instructions, and L <= C + P2 <= 510 never overflows a half, so packed
+ * (P2 <= 255): 1 B/voxel/direction. The sum / WTA kernel adds them up.
+ *
+ * L lanes own a scan line (D = 8 L) and a warp 32 / L lines; a lane owns
+ * eight disparities (four registers of 16-bit pairs; the minima are DPX
+ * instructions, and L_r <= C + P2 <= 510 never overflows a half, so packed
  * adds / subtracts are plain 32-bit ones). The kernel is bound by
  * instruction issue, and the per-step bookkeeping (position, pointers, the
- * shuffle tree of min_k, the loop) costs the same for 256 voxels as it does
- * for 128 with one line per warp; the tree is one level shorter too. A step
- * moves both pointers by a constant (plus or minus one image row where a
- * diagonal wraps around), and the next step's costs are fetched one step
- * ahead. The two lines of a warp are neighbours of the same direction, so
- * they take the same number of steps; a diagonal restarts at different steps
- * on the two, hence no branch around the shuffles: the recurrence is always
- * evaluated and a restarting line overrides it.
+ * shuffle tree of min_k, the loop) costs the same per warp whatever D is,
+ * so every warp carries 256 voxels per step. A step moves both pointers by
+ * a constant (plus or minus one image row where a diagonal wraps around),
+ * and the next step's costs are fetched one step ahead. The lines of a warp
+ * are neighbours of the same direction, so they take the same number of
+ * steps; a diagonal restarts at different steps on each, hence no branch
+ * around the shuffles: the recurrence is always evaluated and a restarting
+ * line overrides it.
  */
+template <int L>
 __global__ void __launch_bounds__(128)
-sgm_paths128_kernel (int w, int h, unsigned P1, unsigned P2,
+sgm_paths_kernel (int w, int h, unsigned P1, unsigned P2,
     uint8_t const* __restrict__ cost, uint8_t* __restrict__ Dvol)
 {
-    constexpr int D = 128;
-    int const pair = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    constexpr int D = 8 * L;
+    constexpr int LPW = 32 / L;                 /* lines per warp */
+    int const grp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     int const lane = threadIdx.x & 31;
-    int const sl = lane & 15;                   /* lane within the line */
-    int const hp = (h + 1) / 2, wp = (w + 1) / 2;
+    int const sl = lane & (L - 1);              /* lane within the line */
+    int const hp = (h + LPW - 1) / LPW, wp = (w + LPW - 1) / LPW;
     int kind, line, count;
-    if (pair < 2 * hp)
+    if (grp < 2 * hp)
     {
-        kind = pair / hp;                       /* PATH_L2R, PATH_R2L */
-        line = 2 * (pair % hp) + (lane >> 4);
+        kind = grp / hp;                        /* PATH_L2R, PATH_R2L */
+        line = LPW * (grp % hp) + (lane >> ilog2(L));
         count = h;
     }
     else
     {
-        int const q = pair - 2 * hp;
+        int const q = grp - 2 * hp;
         if (q >= 6 * wp)
             return;
         kind = 2 + q / wp;                      /* PATH_T2B .. PATH_B2T_D2 */
-        line = 2 * (q % wp) + (lane >> 4);
+        line = LPW * (q % wp) + (lane >> ilog2(L));
         count = w;
     }
-    /* odd line count: the last warp's second half repeats its first line
-     * (it takes part in the shuffles) and stores nothing */
+    /* line count not a multiple of LPW: the leftover lines of the last warp
+     * repeat its last real line (they take part in the shuffles) and store
+     * nothing */
     bool const live = line < count;
     if (!live)
         line = count - 1;
@@ -579,12 +587,12 @@ sgm_paths128_kernel (int w, int h, unsigned P1, unsigned P2,
         unsigned const m2 = __vminu2(__vminu2(Pa, Pb), __vminu2(Pc, Pd));
         unsigned mn = min(m2 & 0xffffu, m2 >> 16);
 #pragma unroll
-        for (int off = 8; off > 0; off >>= 1)
+        for (int off = L / 2; off > 0; off >>= 1)
             mn = min(mn, __shfl_xor_sync(0xffffffffu, mn, off));
         unsigned below = __shfl_up_sync(0xffffffffu, Pd, 1) >> 16;
         unsigned above = __shfl_down_sync(0xffffffffu, Pa, 1) & 0xffffu;
         if (sl == 0) below = BIG;
-        if (sl == 15) above = BIG;
+        if (sl == L - 1) above = BIG;
         unsigned const lo_a = below | (Pa << 16);               /* -, L0 */
         unsigned const ab = __funnelshift_r(Pa, Pb, 16);         /* L1, L2 */
         unsigned const bc = __funnelshift_r(Pb, Pc, 16);         /* L3, L4 */
@@ -615,193 +623,20 @@ sgm_paths128_kernel (int w, int h, unsigned P1, unsigned P2,
     }
 }
 
-template <int DPL>
-__global__ void __launch_bounds__(128)
-sgm_paths_kernel (int w, int h, unsigned P1, unsigned P2,
-    uint8_t const* __restrict__ cost, uint8_t* __restrict__ Dvol)
-{
-    int const D = 32 * DPL;
-    int gw = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-    int const lane = threadIdx.x & 31;
-    int kind, line;
-    if (gw < 2 * h)
-    {
-        kind = gw / h;                  /* PATH_L2R, PATH_R2L */
-        line = gw % h;
-    }
-    else
-    {
-        gw -= 2 * h;
-        if (gw >= 6 * w)
-            return;
-        kind = 2 + gw / w;              /* PATH_T2B .. PATH_B2T_D2 */
-        line = gw % w;
-    }
-    bool const horizontal = (kind < 2);
-    int const steps = horizontal ? w : h;
-    size_t const nvox = static_cast<size_t>(w) * h * D;
-    uint8_t* __restrict__ Dr = Dvol + static_cast<size_t>(kind) * nvox;
-
-    /* start pixel and per-step increments; diagonals wrap around in x,
-     * where the reference restarts the path (:515-534) */
-    int x, y, dx, dy;
-    switch (kind)
-    {
-    case PATH_L2R: x = 0; y = line; dx = 1; dy = 0; break;
-    case PATH_R2L: x = w - 1; y = line; dx = -1; dy = 0; break;
-    case PATH_T2B: x = line; y = 0; dx = 0; dy = 1; break;
-    case PATH_T2B_D1: x = line; y = 0; dx = 1; dy = 1; break;
-    case PATH_T2B_D2: x = line; y = 0; dx = -1; dy = 1; break;
-    case PATH_B2T: x = line; y = h - 1; dx = 0; dy = -1; break;
-    case PATH_B2T_D1: x = line; y = h - 1; dx = 1; dy = -1; break;
-    default: x = line; y = h - 1; dx = -1; dy = -1; break;   /* B2T_D2 */
-    }
-    int const restart_x = (dx > 0) ? 0 : w - 1;   /* diagonals only */
-    bool const diagonal = (!horizontal && dx != 0);
-
-    auto load_cost = [&](size_t base, unsigned* C)
-    {
-#pragma unroll
-        for (int i = 0; i < DPL; ++i) C[i] = cost[base + i];
-    };
-
-    unsigned Lp[DPL], C[DPL];
-#pragma unroll
-    for (int i = 0; i < DPL; ++i) Lp[i] = 0;
-    size_t base = (static_cast<size_t>(y) * w + x) * D + lane * DPL;
-    load_cost(base, C);
-    bool start = true;
-
-    for (int s = 0; s < steps; ++s)
-    {
-        /* next pixel: its cost is fetched while this one is computed */
-        int xn = x + dx, yn = y + dy;
-        if (xn < 0) xn = w - 1;
-        if (xn >= w) xn = 0;
-        bool const startn = diagonal && (xn == restart_x);
-        size_t const basen = (static_cast<size_t>(yn) * w + xn) * D
-            + lane * DPL;
-        unsigned Cn[DPL];
-        if (s + 1 < steps)
-            load_cost(basen, Cn);
-
-        unsigned Dv[DPL];
-        if (start)
-        {
-#pragma unroll
-            for (int i = 0; i < DPL; ++i) { Lp[i] = C[i]; Dv[i] = 0; }
-        }
-        else
-        {
-            unsigned mn = Lp[0];
-#pragma unroll
-            for (int i = 1; i < DPL; ++i) mn = min(mn, Lp[i]);
-            for (int off = 16; off > 0; off >>= 1)
-                mn = min(mn, __shfl_xor_sync(0xffffffffu, mn, off));
-            unsigned const below = __shfl_up_sync(0xffffffffu, Lp[DPL - 1], 1);
-            unsigned const above = __shfl_down_sync(0xffffffffu, Lp[0], 1);
-            unsigned const far = (mn + P2) & 0xffffu;
-            unsigned Ln[DPL];
-#pragma unroll
-            for (int i = 0; i < DPL; ++i)
-            {
-                unsigned best = min(Lp[i], far);
-                bool const has_lo = (i > 0) || (lane > 0);
-                bool const has_hi = (i < DPL - 1) || (lane < 31);
-                unsigned const lo = (i > 0) ? Lp[i - 1] : below;
-                unsigned const hi = (i < DPL - 1) ? Lp[i + 1] : above;
-                if (has_lo) best = min(best, (lo + P1) & 0xffffu);
-                if (has_hi) best = min(best, (hi + P1) & 0xffffu);
-                Dv[i] = (best - mn) & 0xffffu;           /* = L - C, <= P2 */
-                Ln[i] = (C[i] + Dv[i]) & 0xffffu;
-            }
-#pragma unroll
-            for (int i = 0; i < DPL; ++i) Lp[i] = Ln[i];
-        }
-#pragma unroll
-        for (int i = 0; i < DPL; ++i)
-            Dr[base + i] = static_cast<uint8_t>(Dv[i]);
-#pragma unroll
-        for (int i = 0; i < DPL; ++i) C[i] = Cn[i];
-        x = xn; y = yn; base = basen; start = startn;
-    }
-}
-
 /*
  * S(p,i) = sum over the 8 directions of L_r(p,i) = 8 C + sum_r (L_r - C),
  * plus C once more at the four image corners: column 0 of the d1 volume and
  * column w-1 of the d2 volume are (re)initialised for ALL y after row 0 /
  * row h-1 already were (:521-534, :600-613). Then depth_from_sgm_volume
- * (:274-306): first minimum over the planes. One warp per pixel.
- */
-template <int DPL>
-__global__ void
-sgm_sum_wta_kernel (int w, int h, uint8_t const* __restrict__ cost,
-    uint8_t const* __restrict__ Dvol, uint8_t const* __restrict__ main_img,
-    float const* __restrict__ depths, uint16_t* __restrict__ S_out,
-    float* __restrict__ out)
-{
-    int const D = 32 * DPL;
-    int const npix = w * h;
-    int const p = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-    int const lane = threadIdx.x & 31;
-    if (p >= npix)
-        return;
-    size_t const nvox = static_cast<size_t>(npix) * D;
-    size_t const base = static_cast<size_t>(p) * D + lane * DPL;
-    int const px = p % w, py = p / w;
-    unsigned const mult = 8u + (((px == 0 || px == w - 1)
-        && (py == 0 || py == h - 1)) ? 1u : 0u);
-    unsigned Sv[DPL];
-#pragma unroll
-    for (int i = 0; i < DPL; ++i)
-        Sv[i] = (mult * cost[base + i]) & 0xffffu;
-#pragma unroll
-    for (int r = 0; r < 8; ++r)
-    {
-        uint8_t const* Dr = Dvol + r * nvox + base;
-#pragma unroll
-        for (int i = 0; i < DPL; ++i)
-            Sv[i] = (Sv[i] + Dr[i]) & 0xffffu;
-    }
-    if (S_out != nullptr)
-    {
-#pragma unroll
-        for (int i = 0; i < DPL; ++i)
-            S_out[base + i] = static_cast<uint16_t>(Sv[i]);
-    }
-    unsigned best = 0xffffu;    /* numeric_limits<uint16_t>::max() */
-    int best_i = 0;
-    bool found = false;
-#pragma unroll
-    for (int i = 0; i < DPL; ++i)
-        if (Sv[i] < best)
-        {
-            best = Sv[i];
-            best_i = lane * DPL + i;
-            found = true;
-        }
-    /* key = value << 16 | index: min picks the lowest value, then index */
-    unsigned key = found ? ((best << 16) | best_i) : 0xffffffffu;
-    for (int off = 16; off > 0; off >>= 1)
-        key = min(key, __shfl_xor_sync(0xffffffffu, key, off));
-    if (lane == 0)
-    {
-        int const idx = (key == 0xffffffffu) ? 0 : static_cast<int>(
-            key & 0xffffu);
-        out[p] = (idx < 2 || main_img[p] < 25) ? 0.0f : depths[idx];
-    }
-}
-
-/*
- * The same for D = 128 with eight lanes per pixel: a lane owns 16 consecutive
- * disparities and reads them as ONE 16-byte word per volume (nine 128-bit
- * loads per lane instead of 36 byte loads), adds them as pairs of 16-bit
- * fields (S < 9 * 255 + 8 * 255: no carry between the fields), and the
- * argmin -- lowest value, then lowest index, like the reference's first
- * minimum -- runs over the lane's 16 values and then over the pixel's eight
- * lanes. With byte loads the kernel spends its time in the load/store unit
- * (lg_throttle and mio_throttle stalls).
+ * (:274-306): first minimum over the planes.
+ * G = D / 16 lanes per pixel: a lane owns 16 consecutive disparities and
+ * reads them as ONE 16-byte word per volume (nine 128-bit loads per lane
+ * instead of 144 byte loads; with byte loads the kernel spends its time in
+ * the load/store unit, lg_throttle and mio_throttle stalls), adds them as
+ * pairs of 16-bit fields (S <= 9 * 255 + 8 * 255: no carry between the
+ * fields), and the argmin -- lowest value, then lowest index, like the
+ * reference's first minimum -- runs over the lane's 16 values and then over
+ * the pixel's G lanes.
  */
 __device__ __forceinline__ void
 wta_add16 (uint4 const v, unsigned mult, unsigned (&even)[4], unsigned (&odd)[4])
@@ -815,18 +650,20 @@ wta_add16 (uint4 const v, unsigned mult, unsigned (&even)[4], unsigned (&odd)[4]
     }
 }
 
+template <int G>
 __global__ void __launch_bounds__(256)
-sgm_sum_wta128_kernel (int w, int h, uint8_t const* __restrict__ cost,
+sgm_sum_wta_kernel (int w, int h, uint8_t const* __restrict__ cost,
     uint8_t const* __restrict__ Dvol, uint8_t const* __restrict__ main_img,
     float const* __restrict__ depths, uint16_t* __restrict__ S_out,
     float* __restrict__ out)
 {
+    constexpr int D = 16 * G;
     int const npix = w * h;
     int const t = blockIdx.x * blockDim.x + threadIdx.x;
-    int const p = t >> 3, sub = threadIdx.x & 7;
+    int const p = t >> ilog2(G), sub = threadIdx.x & (G - 1);
     bool const on = p < npix;
-    size_t const nvox = static_cast<size_t>(npix) * 128;
-    size_t const base = static_cast<size_t>(on ? p : 0) * 128 + sub * 16;
+    size_t const nvox = static_cast<size_t>(npix) * D;
+    size_t const base = static_cast<size_t>(on ? p : 0) * D + sub * 16;
     int const px = p % w, py = p / w;
     unsigned const mult = 8u + (((px == 0 || px == w - 1)
         && (py == 0 || py == h - 1)) ? 1u : 0u);
@@ -870,9 +707,9 @@ sgm_sum_wta128_kernel (int w, int h, uint8_t const* __restrict__ cost,
                 key = min(key, (val[i] << 16)
                     | static_cast<unsigned>(sub * 16 + k * 4 + i));
     }
-    key = min(key, __shfl_xor_sync(0xffffffffu, key, 4));
-    key = min(key, __shfl_xor_sync(0xffffffffu, key, 2));
-    key = min(key, __shfl_xor_sync(0xffffffffu, key, 1));
+#pragma unroll
+    for (int off = G / 2; off > 0; off >>= 1)
+        key = min(key, __shfl_xor_sync(0xffffffffu, key, off));
     if (sub == 0 && on)
     {
         int const idx = (key == 0xffffffffu) ? 0 : static_cast<int>(
@@ -891,45 +728,22 @@ u8_to_u16_kernel (size_t n, uint8_t const* __restrict__ in,
         out[i] = in[i];
 }
 
-template <int DPL>
+/* K7 and K8 for D planes; mid is recorded between the two launches */
+template <int D>
 void
-run_paths (int w, int h, unsigned P1, unsigned P2, uint8_t const* cost,
-    uint8_t* Dvol, cudaStream_t st)
+run_paths_wta (int w, int h, unsigned P1, unsigned P2, uint8_t const* cost,
+    uint8_t* Dvol, uint8_t const* main_img, float const* depths,
+    uint16_t* S_out, float* out, cudaEvent_t mid, cudaStream_t st)
 {
-    if constexpr (DPL == 4)
-    {
-        /* two lines per warp */
-        int const warps = 2 * ((h + 1) / 2) + 6 * ((w + 1) / 2);
-        sgm_paths128_kernel<<<(warps * 32 + 127) / 128, 128, 0, st>>>(w, h,
-            P1, P2, cost, Dvol);
-    }
-    else
-    {
-        int const warps = 2 * h + 6 * w;
-        sgm_paths_kernel<DPL><<<(warps * 32 + 127) / 128, 128, 0, st>>>(w, h,
-            P1, P2, cost, Dvol);
-    }
+    constexpr int L = D / 8, G = D / 16;        /* lanes per line / pixel */
+    constexpr int LPW = 32 / L;                 /* lines per warp */
+    int const warps = 2 * ((h + LPW - 1) / LPW) + 6 * ((w + LPW - 1) / LPW);
+    sgm_paths_kernel<L><<<(warps * 32 + 127) / 128, 128, 0, st>>>(w, h, P1,
+        P2, cost, Dvol);
     CUDA_CHECK(cudaGetLastError());
-}
-
-template <int DPL>
-void
-run_wta (int w, int h, uint8_t const* cost, uint8_t const* Dvol,
-    uint8_t const* main_img, float const* depths, uint16_t* S_out, float* out,
-    cudaStream_t st)
-{
-    if constexpr (DPL == 4)
-    {
-        int const blocks8 = (w * h * 8 + 255) / 256;
-        sgm_sum_wta128_kernel<<<blocks8, 256, 0, st>>>(w, h, cost, Dvol,
-            main_img, depths, S_out, out);
-    }
-    else
-    {
-        int const blocks = (w * h * 32 + 255) / 256;
-        sgm_sum_wta_kernel<DPL><<<blocks, 256, 0, st>>>(w, h, cost, Dvol,
-            main_img, depths, S_out, out);
-    }
+    CUDA_CHECK(cudaEventRecord(mid, st));
+    sgm_sum_wta_kernel<G><<<(w * h * G + 255) / 256, 256, 0, st>>>(w, h,
+        cost, Dvol, main_img, depths, S_out, out);
     CUDA_CHECK(cudaGetLastError());
 }
 
@@ -1139,22 +953,13 @@ sgm_pair (SgmWorkspace& ws, int w, int h, uint8_t const* main_dev, int nw,
     CUDA_CHECK(cudaGetLastError());
     CUDA_CHECK(cudaEventRecord(ws.ev[e0 + 1], st));
 
-    int const dpl = num_steps / 32;
-    switch (dpl)
-    {
-    case 1: run_paths<1>(w, h, P1, P2, ws.d_cost.p, ws.d_D.p, st); break;
-    case 2: run_paths<2>(w, h, P1, P2, ws.d_cost.p, ws.d_D.p, st); break;
-    case 4: run_paths<4>(w, h, P1, P2, ws.d_cost.p, ws.d_D.p, st); break;
-    default: run_paths<8>(w, h, P1, P2, ws.d_cost.p, ws.d_D.p, st); break;
-    }
-    CUDA_CHECK(cudaEventRecord(ws.ev[e0 + 2], st));
     uint16_t* const S_dev = want_S ? ws.d_S.p : nullptr;
-    switch (dpl)
+    switch (num_steps)
     {
-    case 1: run_wta<1>(w, h, ws.d_cost.p, ws.d_D.p, main_dev, depths_dev, S_dev, out_dev, st); break;
-    case 2: run_wta<2>(w, h, ws.d_cost.p, ws.d_D.p, main_dev, depths_dev, S_dev, out_dev, st); break;
-    case 4: run_wta<4>(w, h, ws.d_cost.p, ws.d_D.p, main_dev, depths_dev, S_dev, out_dev, st); break;
-    default: run_wta<8>(w, h, ws.d_cost.p, ws.d_D.p, main_dev, depths_dev, S_dev, out_dev, st); break;
+    case 32: run_paths_wta<32>(w, h, P1, P2, ws.d_cost.p, ws.d_D.p, main_dev, depths_dev, S_dev, out_dev, ws.ev[e0 + 2], st); break;
+    case 64: run_paths_wta<64>(w, h, P1, P2, ws.d_cost.p, ws.d_D.p, main_dev, depths_dev, S_dev, out_dev, ws.ev[e0 + 2], st); break;
+    case 128: run_paths_wta<128>(w, h, P1, P2, ws.d_cost.p, ws.d_D.p, main_dev, depths_dev, S_dev, out_dev, ws.ev[e0 + 2], st); break;
+    default: run_paths_wta<256>(w, h, P1, P2, ws.d_cost.p, ws.d_D.p, main_dev, depths_dev, S_dev, out_dev, ws.ev[e0 + 2], st); break;
     }
     CUDA_CHECK(cudaEventRecord(ws.ev[e0 + 3], st));
 }
