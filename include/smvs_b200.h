@@ -496,7 +496,9 @@ int smvsb_sgm_reconstruct (int device, int w, int h, const uint8_t* main_lum,
 
 /*
  * MeshGenerator::cut_depth_maps (lib/mesh_generator.cc:25-158): the
- * cross-view consistency cut of all depth maps of a scene, on one device.
+ * cross-view consistency cut of all depth maps of a scene, on one device:
+ * smvsb_cut_depth_maps_multi with the device list { device } and the
+ * default budget.
  *   depth[i]      w[i]*h[i], MVE convention (distance along the viewing ray),
  *                 what View::get_float_image(dm_name) holds (:190)
  *   normals[i]    w[i]*h[i]*3, world space (after :192-203)
@@ -511,6 +513,53 @@ int smvsb_cut_depth_maps (int device, int n_views, const int* w, const int* h,
     const float* const* depth, const float* const* normals,
     const float* invproj9, const float* cam_to_world16, const float* KR9,
     const float* t3, float* const* depth_out);
+
+/* Devices and memory of smvsb_cut_depth_maps_multi. */
+typedef struct smvsb_cut_options
+{
+    const int* devices;          /* one worker per entry; an id may repeat */
+    int32_t n_devices;
+    int32_t reserved0;           /* 0 */
+    uint64_t device_bytes;       /* per device, split among its workers;
+                                    0 = free memory at call time less a
+                                    margin (1/32 of the card, >= 256 MiB) */
+    uint64_t reserved[2];        /* 0 */
+} smvsb_cut_options;
+
+typedef struct smvsb_cut_stats
+{
+    uint64_t reference_pairs;    /* sum of valid pixels x (n_views - 1): the
+                                    (pixel, view) pairs of the reference's loop */
+    uint64_t evaluated_pairs;    /* pairs left after culling */
+    uint64_t bytes_uploaded;     /* host -> device */
+    int32_t target_groups;       /* over all workers */
+    int32_t source_chunks;
+    double ms_device;            /* longest worker, CUDA events */
+} smvsb_cut_stats;
+
+/*
+ * MeshGenerator::cut_depth_maps (lib/mesh_generator.cc:25-158) for scenes
+ * larger than one device, on every device of a list. The maps stay in the
+ * caller's host buffers (as the reference keeps them in host RAM). Each
+ * worker holds a group of target views (as many as its budget holds) and
+ * streams the source views the group needs through pinned staging buffers
+ * in ascending j, chunk by chunk; 16x16 tiles of target pixels skip the
+ * source views their world-space box cannot project into (behind the camera
+ * or outside the image, with fp32 rounding accounted for). Target views come
+ * from a shared counter. The cut maps are those of the reference whatever
+ * the device list, budget, grouping or chunking.
+ *   opts          devices, per-device cap (see smvsb_cut_options)
+ *   stats         may be NULL
+ * Everything else as smvsb_cut_depth_maps. SMVSB_ERR_INVALID: empty device
+ * list, device id out of range, or a device_bytes cap that cannot hold the
+ * largest target view next to one source view; SMVSB_ERR_ALLOC: the device
+ * has not that much free memory.
+ */
+int smvsb_cut_depth_maps_multi (const smvsb_cut_options* opts, int n_views,
+    const int* w, const int* h, const float* const* depth,
+    const float* const* normals, const float* invproj9,
+    const float* cam_to_world16, const float* KR9, const float* t3,
+    float* const* depth_out, smvsb_cut_stats* stats);
 
 #ifdef __cplusplus
 }

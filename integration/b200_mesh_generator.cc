@@ -3,7 +3,8 @@
  *
  * Drop-in body for smvs::MeshGenerator::cut_depth_maps (reference:
  * lib/mesh_generator.cc:25-158): the cross-view consistency cut of all depth
- * maps on the GPU through smvsb_cut_depth_maps. The per-view matrices come
+ * maps on every GPU of the box through smvsb_cut_depth_maps_multi, for scenes
+ * whose maps exceed device memory too. The per-view matrices come
  * from the reference's own camera code (:37-40, :52-58, ViewProjection
  * :302-312); lib/mesh_generator.h is untouched.
  */
@@ -51,9 +52,15 @@ MeshGenerator::cut_depth_maps (std::vector<mve::FloatImage::Ptr> * depthmaps,
         std::copy(this->view_projs[i].t.begin(), this->view_projs[i].t.end(),
             &t[3 * i]);
     }
-    int const rc = smvsb_cut_depth_maps(smvs_b200_integration::thread_device(),
-        static_cast<int>(n), w.data(), h.data(), depth.data(), normals.data(),
-        invproj.data(), ctw.data(), KR.data(), t.data(), out.data());
+    /* every device of the box (or SMVSB_DEVICES), within its free memory:
+     * the maps stay in host RAM, as in the reference */
+    std::vector<int> const& devices = smvs_b200_integration::device_list();
+    smvsb_cut_options opts = {};
+    opts.devices = devices.data();
+    opts.n_devices = static_cast<int>(devices.size());
+    int const rc = smvsb_cut_depth_maps_multi(&opts, static_cast<int>(n),
+        w.data(), h.data(), depth.data(), normals.data(), invproj.data(),
+        ctw.data(), KR.data(), t.data(), out.data(), nullptr);
     if (rc != SMVSB_OK)
         throw std::runtime_error(std::string("smvs_b200: ")
             + smvsb_last_error(nullptr));

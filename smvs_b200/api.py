@@ -29,6 +29,7 @@ EXPORTS = [
     "smvsb_surface_fill_from_depth", "smvsb_surface_remove_isolated", "smvsb_surface_expand", "smvsb_surface_info",
     "smvsb_set_color_images",
     "smvsb_optimize", "smvsb_optimize_rgb_f32", "smvsb_view_set_scale_c", "smvsb_measure_fp64_peak", "smvsb_sgm_reconstruct", "smvsb_newton_loop_batch", "smvsb_device_launch_count",
+    "smvsb_cut_depth_maps_multi",
 ]
 
 
@@ -528,10 +529,26 @@ def optimize(ctx, main_img, sub_imgs, Mi, ti, flen_px, inv_flen, inv_calib9, sgm
     return depth, normals, light, stats
 
 
-def cut_depth_maps(depths, normals, invproj, cam_to_world, KR, t, device=0):
+class CutOptions(C.Structure):
+    _fields_ = [("devices", C.POINTER(C.c_int)), ("n_devices", C.c_int32),
+                ("reserved0", C.c_int32), ("device_bytes", C.c_uint64),
+                ("reserved", C.c_uint64 * 2)]
+
+
+class CutStats(C.Structure):
+    _fields_ = [("reference_pairs", C.c_uint64), ("evaluated_pairs", C.c_uint64),
+                ("bytes_uploaded", C.c_uint64), ("target_groups", C.c_int32),
+                ("source_chunks", C.c_int32), ("ms_device", C.c_double)]
+
+
+def cut_depth_maps(depths, normals, invproj, cam_to_world, KR, t, device=0, *,
+                   devices=None, device_bytes=0, return_stats=False):
     """smvsb_cut_depth_maps: lists of (h, w) depth maps (MVE convention) and
     (h, w, 3) world-space normal maps, per-view matrices as (n, 9) / (n, 16) /
-    (n, 9) / (n, 3) float arrays -> list of cut depth maps."""
+    (n, 9) / (n, 3) float arrays -> list of cut depth maps.
+    devices (a list of ids, one worker each, repeats allowed), device_bytes (a
+    per-device memory cap) or return_stats select smvsb_cut_depth_maps_multi;
+    with return_stats the result is (maps, stats dict)."""
     n = len(depths)
     d = [_f32(a) for a in depths]
     nr = [_f32(a) for a in normals]
@@ -542,8 +559,19 @@ def cut_depth_maps(depths, normals, invproj, cam_to_world, KR, t, device=0):
     npp = (C.c_void_p * n)(*[a.ctypes.data for a in nr])
     op = (C.c_void_p * n)(*[a.ctypes.data for a in outs])
     m = [_f32(a).reshape(-1) for a in (invproj, cam_to_world, KR, t)]
-    rc = lib().smvsb_cut_depth_maps(int(device), n, w, h, dp, npp, _p(m[0]), _p(m[1]),
-                                    _p(m[2]), _p(m[3]), op)
+    args = (n, w, h, dp, npp, _p(m[0]), _p(m[1]), _p(m[2]), _p(m[3]), op)
+    if devices is None and not device_bytes and not return_stats:
+        rc = lib().smvsb_cut_depth_maps(int(device), *args)
+        if rc != 0:
+            raise SmvsbError(rc, lib().smvsb_last_error(None).decode())
+        return outs
+    devs = [int(device)] if devices is None else [int(x) for x in devices]
+    dv = (C.c_int * max(len(devs), 1))(*devs)
+    opts = CutOptions(dv, len(devs), 0, int(device_bytes))
+    st = CutStats()
+    rc = lib().smvsb_cut_depth_maps_multi(C.byref(opts), *args, C.byref(st))
     if rc != 0:
         raise SmvsbError(rc, lib().smvsb_last_error(None).decode())
-    return outs
+    if not return_stats:
+        return outs
+    return outs, {f: getattr(st, f) for f, _ in CutStats._fields_}

@@ -40,10 +40,11 @@ int sgm_run (int device, int w, int h, uint8_t const* main_lum, int nw, int nh,
     uint16_t* sgm_out, double* ms_out);
 double measure_fp64_peak (int device);
 std::string const& cut_last_error (void);
-int cut_depth_maps (int device, int n_views, int const* w, int const* h,
-    float const* const* depth, float const* const* normals,
-    float const* invproj9, float const* cam_to_world16, float const* KR9,
-    float const* t3, float* const* depth_out);
+int cut_depth_maps_multi (smvsb_cut_options const* opts, int n_views,
+    int const* w, int const* h, float const* const* depth,
+    float const* const* normals, float const* invproj9,
+    float const* cam_to_world16, float const* KR9, float const* t3,
+    float* const* depth_out, smvsb_cut_stats* stats);
 int sgm_reconstruct (int device, int w, int h, uint8_t const* main_lum, int nw,
     int nh, uint8_t const* neigh_lum, float const* M_mn, float const* t_mn,
     float const* M_nm, float const* t_nm, float const* depth_range_main,
@@ -1903,8 +1904,22 @@ smvsb_cut_depth_maps (int device, int n_views, const int* w, const int* h,
     const float* invproj9, const float* cam_to_world16, const float* KR9,
     const float* t3, float* const* depth_out)
 {
-    int const rc = smvsb::cut_depth_maps(device, n_views, w, h, depth, normals,
-        invproj9, cam_to_world16, KR9, t3, depth_out);
+    smvsb_cut_options opts = {};
+    opts.devices = &device;
+    opts.n_devices = 1;
+    return smvsb_cut_depth_maps_multi(&opts, n_views, w, h, depth, normals,
+        invproj9, cam_to_world16, KR9, t3, depth_out, nullptr);
+}
+
+int
+smvsb_cut_depth_maps_multi (const smvsb_cut_options* opts, int n_views,
+    const int* w, const int* h, const float* const* depth,
+    const float* const* normals, const float* invproj9,
+    const float* cam_to_world16, const float* KR9, const float* t3,
+    float* const* depth_out, smvsb_cut_stats* stats)
+{
+    int const rc = smvsb::cut_depth_maps_multi(opts, n_views, w, h, depth,
+        normals, invproj9, cam_to_world16, KR9, t3, depth_out, stats);
     if (rc != SMVSB_OK)
         g_last_error = smvsb::cut_last_error();
     return rc;
