@@ -32,25 +32,7 @@ void device_byte_to_float (smvsb_ctx* c, uint8_t const* img_dev, size_t n,
     float* out_dev);
 void device_unpack_texels (smvsb_ctx* c, float const* texels, int n,
     float* grad, float* hess);
-std::string const& sgm_last_error (void);
-int sgm_run (int device, int w, int h, uint8_t const* main_lum, int nw, int nh,
-    uint8_t const* neigh_lum, float const* M, float const* t,
-    float min_depth, float max_depth, int num_steps, uint16_t penalty1,
-    uint16_t penalty2, float* depth_out, uint16_t* cost_out,
-    uint16_t* sgm_out, double* ms_out);
 double measure_fp64_peak (int device);
-std::string const& cut_last_error (void);
-int cut_depth_maps_multi (smvsb_cut_options const* opts, int n_views,
-    int const* w, int const* h, float const* const* depth,
-    float const* const* normals, float const* invproj9,
-    float const* cam_to_world16, float const* KR9, float const* t3,
-    float* const* depth_out, smvsb_cut_stats* stats);
-int sgm_reconstruct (int device, int w, int h, uint8_t const* main_lum, int nw,
-    int nh, uint8_t const* neigh_lum, float const* M_mn, float const* t_mn,
-    float const* M_nm, float const* t_nm, float const* depth_range_main,
-    float const* depth_range_neigh, int num_steps, uint16_t penalty1,
-    uint16_t penalty2, float const* merge_with, float* depth_out,
-    double* ms_out);
 }
 
 namespace smvsb {
@@ -240,6 +222,66 @@ pseudo_inverse_16 (double const* A, double* Ainv)
                 s += V[i * N + k] * sinv[k] * U[j * N + k];
             Ainv[i * N + j] = s;
         }
+}
+
+/* The lighting parameters from the normal equations Ab = A (16x16) | b (16):
+ * pinv(A) b (lib/light_optimizer.cc:50-52). */
+void
+lighting_from_normal_equations (double const* Ab, double* out16)
+{
+    double Ainv[256];
+    pseudo_inverse_16(Ab, Ainv);
+    for (int i = 0; i < 16; ++i)
+    {
+        double s = 0.0;
+        for (int j = 0; j < 16; ++j)
+            s += Ainv[i * 16 + j] * Ab[256 + j];
+        out16[i] = s;
+    }
+}
+
+/* New views for the context: the stored grid and visibility ids were checked
+ * against the old image size and neighbour count. The colour images
+ * (smvsb_set_color_images) stay while the geometry of the views does: the
+ * reference's get_image() does not change with the scale. */
+void
+forget_stale_views (smvsb_ctx* c, int w, int h, int n_sub, int const* sub_w,
+    int const* sub_h)
+{
+    if (c->w != w || c->h != h || c->n_sub != n_sub)
+    {
+        c->have_surface = false;
+        c->have_color = false;
+    }
+    for (int k = 0; c->have_color && k < n_sub; ++k)
+        if (c->subs[k].w != sub_w[k] || c->subs[k].h != sub_h[k])
+            c->have_color = false;
+}
+
+/* The neighbour tables from arguments the caller checked: each neighbour's
+ * size and texel buffer (reserved; the caller fills it), and the device
+ * arrays of texel pointers, sizes and M | t that the kernels read. */
+void
+set_neighbour_tables (smvsb_ctx* c, int n_sub, int const* sub_w,
+    int const* sub_h, double const* Mi, double const* ti)
+{
+    c->n_sub = n_sub;
+    std::vector<float const*> ptrs(std::max(n_sub, 1), nullptr);
+    std::vector<int> dims(std::max(2 * n_sub, 2), 0);
+    std::vector<double> mt(std::max(12 * n_sub, 12), 0.0);
+    for (int k = 0; k < n_sub; ++k)
+    {
+        smvsb::SubViewDev& sv = c->subs[k];
+        sv.w = sub_w[k]; sv.h = sub_h[k];
+        sv.texels.reserve(static_cast<size_t>(sv.w) * sv.h * SMVSB_NB_STRIDE);
+        ptrs[k] = sv.texels.p;
+        dims[2 * k] = sv.w; dims[2 * k + 1] = sv.h;
+        std::copy(Mi + 9 * k, Mi + 9 * k + 9, mt.begin() + 12 * k);
+        std::copy(ti + 3 * k, ti + 3 * k + 3, mt.begin() + 12 * k + 9);
+    }
+    upload(c, c->sub_ptrs, ptrs.data(), ptrs.size());
+    upload(c, c->sub_dims, dims.data(), dims.size());
+    upload(c, c->Mt, mt.data(), mt.size());
 }
 
 void
@@ -464,12 +506,7 @@ smvsb_measure_fp64_peak (int device, double* tflops_out)
 {
     return guarded(nullptr, [&]() {
         require(tflops_out != nullptr, SMVSB_ERR_INVALID, "NULL output");
-        int count = 0;
-        if (cudaGetDeviceCount(&count) != cudaSuccess || count == 0)
-            throw smvsb::Error(SMVSB_ERR_CUDA,
-                "no CUDA device (smvs_b200 has no CPU fallback)");
-        require(device >= 0 && device < count, SMVSB_ERR_INVALID,
-            "device index out of range");
+        smvsb::check_device(device);
         *tflops_out = smvsb::measure_fp64_peak(device);
     });
 }
@@ -480,14 +517,7 @@ smvsb_create (int device, smvsb_ctx** out)
     return guarded(nullptr, [&]() {
         require(out != nullptr, SMVSB_ERR_INVALID, "out must not be NULL");
         *out = nullptr;
-        int count = 0;
-        cudaError_t e = cudaGetDeviceCount(&count);
-        if (e != cudaSuccess || count == 0)
-            throw smvsb::Error(SMVSB_ERR_CUDA, std::string("no CUDA device "
-                "(smvs_b200 has no CPU fallback): ")
-                + cudaGetErrorString(e));
-        require(device >= 0 && device < count, SMVSB_ERR_INVALID,
-            "device index out of range");
+        smvsb::check_device(device);
         CUDA_CHECK(cudaSetDevice(device));
         smvsb_ctx* c = new smvsb_ctx();
         c->device = device;
@@ -508,11 +538,11 @@ smvsb_create (int device, smvsb_ctx** out)
             }
             CUDA_CHECK(cudaDeviceGetAttribute(&c->num_sms,
                 cudaDevAttrMultiProcessorCount, device));
-            CUDA_CHECK(cudaMallocHost(&c->h_scalars, 32 * sizeof(double)));
+            CUDA_CHECK(cudaMallocHost(&c->pinned, sizeof(*c->pinned)));
         }
         catch (...)
         {
-            if (c->h_scalars) cudaFreeHost(c->h_scalars);
+            if (c->pinned) cudaFreeHost(c->pinned);
             for (int i = 0; i < 2; ++i)
             {
                 if (c->ev_copied[i]) cudaEventDestroy(c->ev_copied[i]);
@@ -546,7 +576,7 @@ smvsb_destroy (smvsb_ctx* ctx)
     }
     if (ctx->copy_stream) cudaStreamDestroy(ctx->copy_stream);
     if (ctx->stream) cudaStreamDestroy(ctx->stream);
-    if (ctx->h_scalars) cudaFreeHost(ctx->h_scalars);
+    if (ctx->pinned) cudaFreeHost(ctx->pinned);
     delete ctx;
 }
 
@@ -567,19 +597,11 @@ smvsb_set_views (smvsb_ctx* ctx, int w, int h, double flen_px,
             SMVSB_ERR_INVALID, "shading image and gradient go together");
         require(n_sub == 0 || (sub_w && sub_h && sub_grad && sub_hess && Mi
             && ti), SMVSB_ERR_INVALID, "neighbour arrays missing");
+        for (int k = 0; k < n_sub; ++k)
+            require(sub_w[k] > 0 && sub_h[k] > 0 && sub_grad[k]
+                && sub_hess[k], SMVSB_ERR_INVALID, "neighbour image missing");
         smvsb_ctx* c = ctx;
-        /* the stored grid and visibility ids were checked against the old
-         * image size and neighbour count */
-        if (c->w != w || c->h != h || c->n_sub != n_sub)
-            c->have_surface = false;
-        /* colour images (smvsb_set_color_images) stay while the geometry of
-         * the views does: the reference's get_image() does not change with
-         * the scale */
-        if (c->w != w || c->h != h || c->n_sub != n_sub)
-            c->have_color = false;
-        for (int k = 0; c->have_color && k < n_sub; ++k)
-            if (c->subs[k].w != sub_w[k] || c->subs[k].h != sub_h[k])
-                c->have_color = false;
+        forget_stale_views(c, w, h, n_sub, sub_w, sub_h);
         c->w = w; c->h = h; c->flen = flen_px; c->inv_flen = inv_flen;
         size_t const npix = static_cast<size_t>(w) * h;
         upload(c, c->main_grad, main_grad, npix * 2);
@@ -589,32 +611,18 @@ smvsb_set_views (smvsb_ctx* ctx, int w, int h, double flen_px,
             upload(c, c->main_shading, main_shading, npix);
             upload(c, c->main_shading_grad, main_shading_grad, npix * 2);
         }
-        c->n_sub = n_sub;
-        std::vector<float const*> ptrs(std::max(n_sub, 1), nullptr);
-        std::vector<int> dims(std::max(2 * n_sub, 2), 0);
-        std::vector<double> mt(std::max(12 * n_sub, 12), 0.0);
+        set_neighbour_tables(c, n_sub, sub_w, sub_h, Mi, ti);
         smvsb::DevBuf<float>& stage_g = c->stage_a;
         smvsb::DevBuf<float>& stage_h = c->stage_b;
         for (int k = 0; k < n_sub; ++k)
         {
-            require(sub_w[k] > 0 && sub_h[k] > 0 && sub_grad[k]
-                && sub_hess[k], SMVSB_ERR_INVALID, "neighbour image missing");
-            size_t const n = static_cast<size_t>(sub_w[k]) * sub_h[k];
             smvsb::SubViewDev& sv = c->subs[k];
-            sv.w = sub_w[k]; sv.h = sub_h[k];
-            sv.texels.reserve(n * SMVSB_NB_STRIDE);
+            size_t const n = static_cast<size_t>(sv.w) * sv.h;
             upload(c, stage_g, sub_grad[k], n * 2);
             upload(c, stage_h, sub_hess[k], n * 3);
             smvsb::launch_pack_subview(c, stage_g.p, stage_h.p, sv.texels.p,
                 sv.w, sv.h);
-            ptrs[k] = sv.texels.p;
-            dims[2 * k] = sv.w; dims[2 * k + 1] = sv.h;
-            std::copy(Mi + 9 * k, Mi + 9 * k + 9, mt.begin() + 12 * k);
-            std::copy(ti + 3 * k, ti + 3 * k + 3, mt.begin() + 12 * k + 9);
         }
-        upload(c, c->sub_ptrs, ptrs.data(), ptrs.size());
-        upload(c, c->sub_dims, dims.data(), dims.size());
-        upload(c, c->Mt, mt.data(), mt.size());
         CUDA_CHECK(cudaStreamSynchronize(c->stream));   /* staging buffers */
         c->have_views = true;
         c->have_system = false;
@@ -637,18 +645,6 @@ smvsb_set_views_u8 (smvsb_ctx* ctx, int scale, int w, int h, double flen_px,
             "n_sub out of range (max 32)");
         require(n_sub == 0 || (sub_w && sub_h && sub_img && Mi && ti),
             SMVSB_ERR_INVALID, "neighbour arrays missing");
-        smvsb_ctx* c = ctx;
-        if (c->w != w || c->h != h || c->n_sub != n_sub)
-            c->have_surface = false;
-        /* colour images (smvsb_set_color_images) stay while the geometry of
-         * the views does: the reference's get_image() does not change with
-         * the scale */
-        if (c->w != w || c->h != h || c->n_sub != n_sub)
-            c->have_color = false;
-        for (int k = 0; c->have_color && k < n_sub; ++k)
-            if (c->subs[k].w != sub_w[k] || c->subs[k].h != sub_h[k])
-                c->have_color = false;
-        c->w = w; c->h = h; c->flen = flen_px; c->inv_flen = inv_flen;
         size_t max_pix = static_cast<size_t>(w) * h;
         for (int k = 0; k < n_sub; ++k)
         {
@@ -657,6 +653,10 @@ smvsb_set_views_u8 (smvsb_ctx* ctx, int scale, int w, int h, double flen_px,
             max_pix = std::max(max_pix, static_cast<size_t>(sub_w[k])
                 * sub_h[k]);
         }
+        smvsb_ctx* c = ctx;
+        forget_stale_views(c, w, h, n_sub, sub_w, sub_h);
+        c->w = w; c->h = h; c->flen = flen_px; c->inv_flen = inv_flen;
+        set_neighbour_tables(c, n_sub, sub_w, sub_h, Mi, ti);
         c->stage_u8.reserve(max_pix);
         c->stage_u8b.reserve(max_pix);
         c->stage_a.reserve(max_pix);
@@ -704,16 +704,9 @@ smvsb_set_views_u8 (smvsb_ctx* ctx, int scale, int w, int h, double flen_px,
             }
             release(0);
         }
-        c->n_sub = n_sub;
-        std::vector<float const*> ptrs(std::max(n_sub, 1), nullptr);
-        std::vector<int> dims(std::max(2 * n_sub, 2), 0);
-        std::vector<double> mt(std::max(12 * n_sub, 12), 0.0);
         for (int k = 0; k < n_sub; ++k)
         {
             smvsb::SubViewDev& sv = c->subs[k];
-            sv.w = sub_w[k]; sv.h = sub_h[k];
-            sv.texels.reserve(static_cast<size_t>(sv.w) * sv.h
-                * SMVSB_NB_STRIDE);
             if (k + 1 < n_sub)
                 stage_image(k + 2, sub_img[k + 1],
                     static_cast<size_t>(sub_w[k + 1]) * sub_h[k + 1]);
@@ -721,14 +714,7 @@ smvsb_set_views_u8 (smvsb_ctx* ctx, int scale, int w, int h, double flen_px,
             smvsb::device_set_scale(c, src, sv.w, sv.h, scale,
                 c->stage_a.p, c->stage_b.p, 1, sv.texels.p);
             release(k + 1);
-            ptrs[k] = sv.texels.p;
-            dims[2 * k] = sv.w; dims[2 * k + 1] = sv.h;
-            std::copy(Mi + 9 * k, Mi + 9 * k + 9, mt.begin() + 12 * k);
-            std::copy(ti + 3 * k, ti + 3 * k + 3, mt.begin() + 12 * k + 9);
         }
-        upload(c, c->sub_ptrs, ptrs.data(), ptrs.size());
-        upload(c, c->sub_dims, dims.data(), dims.size());
-        upload(c, c->Mt, mt.data(), mt.size());
         CUDA_CHECK(cudaStreamSynchronize(c->stream));
         c->have_views = true;
         c->have_system = false;
@@ -919,14 +905,13 @@ smvsb_set_surface (smvsb_ctx* ctx, int scale, int npx, int npy, int start_x,
             c->vis_off.p, c->vis_ids.p, c->counters.p);
         smvsb::count_launches(c, 1);
         CUDA_CHECK(cudaGetLastError());
-        CUDA_CHECK(cudaMemcpyAsync(c->h_scalars + 16, c->counters.p,
+        CUDA_CHECK(cudaMemcpyAsync(&c->pinned->vis_flags, c->counters.p,
             sizeof(unsigned long long), cudaMemcpyDeviceToHost, c->stream));
         c->h_node_valid.assign(node_valid, node_valid + c->n_nodes);
         c->h_patch_valid.assign(patch_valid, patch_valid + c->n_patches);
         set_active(c, nullptr);
         CUDA_CHECK(cudaStreamSynchronize(c->stream));
-        unsigned long long bad = 0;
-        std::memcpy(&bad, c->h_scalars + 16, sizeof(bad));
+        unsigned long long const bad = c->pinned->vis_flags;
         require(!(bad & 1u), SMVSB_ERR_INVALID, "vis_off must be monotone");
         require(!(bad & 2u), SMVSB_ERR_INVALID,
             "visibility list longer than the number of neighbours");
@@ -1333,28 +1318,28 @@ optimize_resident (smvsb_ctx* ctx, int w, int h, double flen_px,
             "use_shading needs the shading image");
         require(opts->num_iterations >= 1 && opts->min_scale >= 0,
             SMVSB_ERR_INVALID, "bad iteration count / min_scale");
+        for (int k = 0; k < n_sub; ++k)
+            require(sub_w[k] > 2 && sub_h[k] > 2 && sub_img[k],
+                SMVSB_ERR_INVALID, "neighbour image missing");
         smvsb_optimize_stats st;
         std::memset(&st, 0, sizeof(st));
 
         /* ---- inputs: once per view ------------------------------------ */
         c->w = w; c->h = h; c->flen = flen_px; c->inv_flen = inv_flen;
-        c->n_sub = n_sub;
+        /* the surface and the colour images are made anew, whatever the
+         * geometry of the views */
         c->have_surface = false;
-        size_t const npix = static_cast<size_t>(w) * h;
         c->have_color = false;
+        set_neighbour_tables(c, n_sub, sub_w, sub_h, Mi, ti);
+        size_t const npix = static_cast<size_t>(w) * h;
         if (colour)
             upload(c, c->color_main, static_cast<float const*>(main_img),
                 npix * 3);
         else
             upload(c, c->u8_main, static_cast<uint8_t const*>(main_img), npix);
         std::vector<float const*> colour_ptrs(n_sub, nullptr);
-        std::vector<float const*> ptrs(n_sub, nullptr);
-        std::vector<int> dims(2 * n_sub, 0);
-        std::vector<double> mt(12 * n_sub, 0.0);
         for (int k = 0; k < n_sub; ++k)
         {
-            require(sub_w[k] > 2 && sub_h[k] > 2 && sub_img[k],
-                SMVSB_ERR_INVALID, "neighbour image missing");
             size_t const n = static_cast<size_t>(sub_w[k]) * sub_h[k];
             if (colour)
             {
@@ -1365,17 +1350,7 @@ optimize_resident (smvsb_ctx* ctx, int w, int h, double flen_px,
             else
                 upload(c, c->u8_subs[k],
                     static_cast<uint8_t const*>(sub_img[k]), n);
-            smvsb::SubViewDev& sv = c->subs[k];
-            sv.w = sub_w[k]; sv.h = sub_h[k];
-            sv.texels.reserve(n * SMVSB_NB_STRIDE);
-            ptrs[k] = sv.texels.p;
-            dims[2 * k] = sv.w; dims[2 * k + 1] = sv.h;
-            std::copy(Mi + 9 * k, Mi + 9 * k + 9, mt.begin() + 12 * k);
-            std::copy(ti + 3 * k, ti + 3 * k + 3, mt.begin() + 12 * k + 9);
         }
-        upload(c, c->sub_ptrs, ptrs.data(), ptrs.size());
-        upload(c, c->sub_dims, dims.data(), dims.size());
-        upload(c, c->Mt, mt.data(), mt.size());
         if (colour)
         {
             upload(c, c->color_ptrs, colour_ptrs.data(), colour_ptrs.size());
@@ -1432,6 +1407,15 @@ optimize_resident (smvsb_ctx* ctx, int w, int h, double flen_px,
 
         bool have_light = false;
         double light[16];
+        /* cut_boundaries until it deletes at most 10 patches */
+        auto cut_until_settled = [&]()
+        {
+            for (uint64_t del = ~0ull; del > 10;)
+            {
+                del = smvsb::run_cut_boundaries(c, inv_calib9);
+                refresh_validity(c);
+            }
+        };
         auto run_newton_iterations = [&]()
         {
             bool finished = false;
@@ -1446,11 +1430,7 @@ optimize_resident (smvsb_ctx* ctx, int w, int h, double flen_px,
                     else
                         smvsb::run_visibility_device(c);
                     refresh_validity(c);
-                    for (uint64_t del = ~0ull; del > 10;)
-                    {
-                        del = smvsb::run_cut_boundaries(c, inv_calib9);
-                        refresh_validity(c);
-                    }
+                    cut_until_settled();
                 }
                 smvsb_newton_stats ns;
                 smvsb_ctx* cs[1] = { c };
@@ -1466,11 +1446,7 @@ optimize_resident (smvsb_ctx* ctx, int w, int h, double flen_px,
                 if (finished)
                     break;
                 /* :322-356 */
-                for (uint64_t del = ~0ull; del > 10;)
-                {
-                    del = smvsb::run_cut_boundaries(c, inv_calib9);
-                    refresh_validity(c);
-                }
+                cut_until_settled();
                 if (no_sgm)
                 {
                     /* :331-339: grow the surface by a ring of patches, see
@@ -1479,11 +1455,7 @@ optimize_resident (smvsb_ctx* ctx, int w, int h, double flen_px,
                     refresh_validity(c);
                     smvsb::run_visibility_ncc(c);
                     refresh_validity(c);
-                    for (uint64_t del = ~0ull; del > 10;)
-                    {
-                        del = smvsb::run_cut_boundaries(c, inv_calib9);
-                        refresh_validity(c);
-                    }
+                    cut_until_settled();
                 }
                 smvsb::topo_remove_isolated(c);
                 refresh_validity(c);
@@ -1507,16 +1479,9 @@ optimize_resident (smvsb_ctx* ctx, int w, int h, double flen_px,
             refresh_validity(c);
             if (opts->use_shading && c->scale < 4)           /* :102-109 */
             {
-                double Ab[272], Ainv[256];
+                double Ab[272];
                 smvsb::run_fit_lighting(c, Ab);
-                pseudo_inverse_16(Ab, Ainv);
-                for (int i = 0; i < 16; ++i)
-                {
-                    double acc = 0.0;
-                    for (int j = 0; j < 16; ++j)
-                        acc += Ainv[i * 16 + j] * Ab[256 + j];
-                    light[i] = acc;
-                }
+                lighting_from_normal_equations(Ab, light);
                 have_light = true;
             }
             run_newton_iterations();
@@ -1849,15 +1814,7 @@ smvsb_fit_lighting (smvsb_ctx* ctx, double* params16_out, void* nccl_comm)
             require(rc == 0, SMVSB_ERR_CUDA, "ncclAllReduce failed");
             download(c, Ab, c->light_partials.p, 272);
         }
-        double Ainv[256];
-        pseudo_inverse_16(Ab, Ainv);
-        for (int i = 0; i < 16; ++i)
-        {
-            double s = 0.0;
-            for (int j = 0; j < 16; ++j)
-                s += Ainv[i * 16 + j] * Ab[256 + j];
-            params16_out[i] = s;
-        }
+        lighting_from_normal_equations(Ab, params16_out);
     });
 }
 
@@ -1868,15 +1825,11 @@ smvsb_sgm (int device, int w, int h, const uint8_t* main_lum, int nw, int nh,
     uint16_t penalty2, float* depth_out, uint16_t* cost_out,
     uint16_t* sgm_out, double* ms_out)
 {
-    int const rc = smvsb::sgm_run(device, w, h, main_lum, nw, nh, neigh_lum,
-        M, t, min_depth, max_depth, num_steps, penalty1, penalty2, depth_out,
-        cost_out, sgm_out, ms_out);
-    if (rc != SMVSB_OK)
-        g_last_error = smvsb::sgm_last_error();
-    else
-        smvsb::count_device_launches(device, 3);   /* cost volume, 8-path
-                                           aggregation, sum + WTA */
-    return rc;
+    return guarded(nullptr, [&]() {
+        smvsb::sgm_run(device, w, h, main_lum, nw, nh, neigh_lum, M, t,
+            min_depth, max_depth, num_steps, penalty1, penalty2, depth_out,
+            cost_out, sgm_out, ms_out);
+    });
 }
 
 int
@@ -1887,15 +1840,11 @@ smvsb_sgm_reconstruct (int device, int w, int h, const uint8_t* main_lum,
     int num_steps, uint16_t penalty1, uint16_t penalty2,
     const float* merge_with, float* depth_out, double* ms_out)
 {
-    int const rc = smvsb::sgm_reconstruct(device, w, h, main_lum, nw, nh,
-        neigh_lum, M_mn, t_mn, M_nm, t_nm, depth_range_main,
-        depth_range_neigh, num_steps, penalty1, penalty2, merge_with,
-        depth_out, ms_out);
-    if (rc != SMVSB_OK)
-        g_last_error = smvsb::sgm_last_error();
-    else    /* 2 x (cost, paths, WTA) + consistency (+ merge) */
-        smvsb::count_device_launches(device, merge_with ? 8 : 7);
-    return rc;
+    return guarded(nullptr, [&]() {
+        smvsb::sgm_reconstruct(device, w, h, main_lum, nw, nh, neigh_lum,
+            M_mn, t_mn, M_nm, t_nm, depth_range_main, depth_range_neigh,
+            num_steps, penalty1, penalty2, merge_with, depth_out, ms_out);
+    });
 }
 
 int
@@ -1918,11 +1867,10 @@ smvsb_cut_depth_maps_multi (const smvsb_cut_options* opts, int n_views,
     const float* cam_to_world16, const float* KR9, const float* t3,
     float* const* depth_out, smvsb_cut_stats* stats)
 {
-    int const rc = smvsb::cut_depth_maps_multi(opts, n_views, w, h, depth,
-        normals, invproj9, cam_to_world16, KR9, t3, depth_out, stats);
-    if (rc != SMVSB_OK)
-        g_last_error = smvsb::cut_last_error();
-    return rc;
+    return guarded(nullptr, [&]() {
+        smvsb::cut_depth_maps_multi(opts, n_views, w, h, depth, normals,
+            invproj9, cam_to_world16, KR9, t3, depth_out, stats);
+    });
 }
 
 } /* extern "C" */

@@ -67,7 +67,6 @@
  * of a CTA then stream separate pieces of H instead of one contiguous piece).
  */
 #include <algorithm>
-#include <cstring>
 
 #include "common.cuh"
 
@@ -1127,9 +1126,9 @@ cg_enqueue (smvsb_ctx* const* cs, int n, int max_iter, double err_tol,
     for (int k = 0; k < n; ++k)
     {
         smvsb_ctx* c = cs[k];
-        CUDA_CHECK(cudaMemcpyAsync(c->h_scalars, c->cg_result.p,
+        CUDA_CHECK(cudaMemcpyAsync(c->pinned->cg, c->cg_result.p,
             3 * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
-        CUDA_CHECK(cudaMemcpyAsync(c->h_scalars + 8, c->cg_counts.p,
+        CUDA_CHECK(cudaMemcpyAsync(c->pinned->cg_counts, c->cg_counts.p,
             2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost,
             c->stream));
     }
@@ -1138,11 +1137,9 @@ cg_enqueue (smvsb_ctx* const* cs, int n, int max_iter, double err_tol,
 void
 cg_collect (smvsb_ctx* c, int* iters, int* info, bool* x0_nan)
 {
-    double const* res = c->h_scalars;
-    unsigned long long counts[2];
-    std::memcpy(counts, c->h_scalars + 8, sizeof(counts));
-    c->cg_blocks = counts[0];
-    c->cg_rows = counts[1];
+    double const* res = c->pinned->cg;
+    c->cg_blocks = c->pinned->cg_counts[0];
+    c->cg_rows = c->pinned->cg_counts[1];
     if (iters) *iters = static_cast<int>(res[0]);
     if (info) *info = static_cast<int>(res[1]);
     if (x0_nan) *x0_nan = (res[2] != 0.0);

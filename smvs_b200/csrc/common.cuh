@@ -99,6 +99,18 @@ struct SurfaceDev
     double const* basis_f;              /* all pixel positions: 3 * ps * 4 */
 };
 
+/* Page-locked landing places of a context's asynchronous read-backs: each is
+ * copied on the context's stream and read after that stream synchronised. */
+struct PinnedResults
+{
+    double cg[3];                       /* cg_result: iterations, info, x0 NaN */
+    unsigned long long cg_counts[2];    /* blocks, rows of the solved system */
+    double update[3];                   /* upd_result: shift sum, shift count,
+                                           active nodes */
+    unsigned long long processed;       /* patches count_processed counted */
+    unsigned long long vis_flags;       /* smvsb_set_surface's list check */
+};
+
 } /* namespace smvsb */
 
 struct smvsb_ctx
@@ -168,8 +180,7 @@ struct smvsb_ctx
     smvsb::DevBuf<uint32_t> cg_row_list, cg_block_rows;
     smvsb::DevBuf<unsigned long long> cg_counts;
     uint64_t cg_blocks = 0, cg_rows = 0;    /* of the last solve's system */
-    double* h_scalars = nullptr;        /* pinned, 32 doubles: results of the
-                                           asynchronous read-backs */
+    smvsb::PinnedResults* pinned = nullptr;
     smvsb::DevBuf<unsigned int> cg_sync;
     smvsb::DevBuf<double> cg_result;    /* iters, info, ... */
 
@@ -220,6 +231,23 @@ count_launches (smvsb_ctx* c, int n)
 {
     c->launches += n;
     count_device_launches(c->device, n);
+}
+
+/* Throws unless `device` names a CUDA device of this process. */
+inline void
+check_device (int device)
+{
+    int count = 0;
+    cudaError_t const e = cudaGetDeviceCount(&count);
+    if (e != cudaSuccess || count == 0)
+    {
+        cudaGetLastError();
+        throw Error(SMVSB_ERR_CUDA, std::string("no CUDA device "
+            "(smvs_b200 has no CPU fallback)") + (e != cudaSuccess
+            ? std::string(": ") + cudaGetErrorString(e) : std::string()));
+    }
+    if (device < 0 || device >= count)
+        throw Error(SMVSB_ERR_INVALID, "device index out of range");
 }
 
 inline SurfaceDev
@@ -280,6 +308,22 @@ void topo_remove_isolated (smvsb_ctx* c);
 uint64_t topo_expand (smvsb_ctx* c);
 uint64_t topo_count_patches (smvsb_ctx* c);
 uint64_t run_cut_boundaries (smvsb_ctx* c, float const* inv_calib9);
+void sgm_run (int device, int w, int h, uint8_t const* main_lum, int nw, int nh,
+    uint8_t const* neigh_lum, float const* M, float const* t,
+    float min_depth, float max_depth, int num_steps, uint16_t penalty1,
+    uint16_t penalty2, float* depth_out, uint16_t* cost_out,
+    uint16_t* sgm_out, double* ms_out);
+void sgm_reconstruct (int device, int w, int h, uint8_t const* main_lum,
+    int nw, int nh, uint8_t const* neigh_lum, float const* M_mn,
+    float const* t_mn, float const* M_nm, float const* t_nm,
+    float const* depth_range_main, float const* depth_range_neigh,
+    int num_steps, uint16_t penalty1, uint16_t penalty2,
+    float const* merge_with, float* depth_out, double* ms_out);
+void cut_depth_maps_multi (smvsb_cut_options const* opts, int n_views,
+    int const* w, int const* h, float const* const* depth,
+    float const* const* normals, float const* invproj9,
+    float const* cam_to_world16, float const* KR9, float const* t3,
+    float* const* depth_out, smvsb_cut_stats* stats);
 
 } /* namespace smvsb */
 

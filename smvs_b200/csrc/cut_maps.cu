@@ -459,7 +459,6 @@ cut_finalize_kernel (CutTarget const T)
 }
 
 std::mutex g_cut_lock;
-thread_local std::string g_cut_error;
 
 constexpr size_t kAlign = 256;
 
@@ -627,6 +626,7 @@ private:
 
     void upload (int v, float* d_cut, float* d_nrm, float* d_z,
         cudaEvent_t wait);
+    CutTarget cut_target (Target const& T) const;
     void run_group (std::vector<int> const& group);
 
     Scene& S;
@@ -671,6 +671,18 @@ Worker::upload (int v, float* d_cut, float* d_nrm, float* d_z,
     CUDA_CHECK(cudaGetLastError());
     stats.bytes += 16 * n;
     stats.launches += 1;
+}
+
+/* The chunk and finalize kernels' view of a target of the group. */
+CutTarget
+Worker::cut_target (Target const& T) const
+{
+    CutTarget ct;
+    S.fill_view(T.i, &ct.v);
+    ct.v.cut = T.cut; ct.v.zdepth = T.z; ct.v.normals = T.nrm;
+    ct.acc = T.acc; ct.done = T.done; ct.keep = T.keep;
+    ct.nwords = S.nwords; ct.tiles_x = S.tiles_x(T.i);
+    return ct;
 }
 
 void
@@ -894,14 +906,9 @@ Worker::run_group (std::vector<int> const& group)
             if (!any)
                 continue;
             int const i = T.i;
-            CutTarget ct;
-            S.fill_view(i, &ct.v);
-            ct.v.cut = T.cut; ct.v.zdepth = T.z; ct.v.normals = T.nrm;
-            ct.acc = T.acc; ct.done = T.done; ct.keep = T.keep;
-            ct.nwords = nw; ct.tiles_x = S.tiles_x(i);
             dim3 const grid(S.tiles_x(i), (S.h[i] + kTile - 1) / kTile);
-            cut_chunk_kernel<<<grid, dim3(kTile, kTile), 0, st>>>(ct,
-                d_views, i, j0, j1);
+            cut_chunk_kernel<<<grid, dim3(kTile, kTile), 0, st>>>(
+                cut_target(T), d_views, i, j0, j1);
             CUDA_CHECK(cudaGetLastError());
             stats.launches += 1;
         }
@@ -912,13 +919,9 @@ Worker::run_group (std::vector<int> const& group)
     for (Target const& T : tg)
     {
         int const i = T.i;
-        CutTarget ct;
-        S.fill_view(i, &ct.v);
-        ct.v.cut = T.cut; ct.v.zdepth = T.z; ct.v.normals = T.nrm;
-        ct.acc = T.acc; ct.done = T.done; ct.keep = T.keep;
-        ct.nwords = nw; ct.tiles_x = S.tiles_x(i);
         dim3 const grid(S.tiles_x(i), (S.h[i] + kTile - 1) / kTile);
-        cut_finalize_kernel<<<grid, dim3(kTile, kTile), 0, st>>>(ct);
+        cut_finalize_kernel<<<grid, dim3(kTile, kTile), 0, st>>>(
+            cut_target(T));
         CUDA_CHECK(cudaGetLastError());
         stats.launches += 1;
         CUDA_CHECK(cudaMemcpyAsync(S.out[i], T.acc, S.pix(i) * sizeof(float),
@@ -929,100 +932,92 @@ Worker::run_group (std::vector<int> const& group)
 
 } /* namespace */
 
-std::string const&
-cut_last_error (void)
-{
-    return g_cut_error;
-}
-
-int
+void
 cut_depth_maps_multi (smvsb_cut_options const* opts, int n_views,
     int const* w, int const* h, float const* const* depth,
     float const* const* normals, float const* invproj9,
     float const* cam_to_world16, float const* KR9, float const* t3,
     float* const* depth_out, smvsb_cut_stats* stats)
 {
-    int rc = SMVSB_OK;
-    try
-    {
-        if (n_views < 1 || !w || !h || !depth || !normals || !invproj9
-            || !cam_to_world16 || !KR9 || !t3 || !depth_out || !opts)
-            throw Error(SMVSB_ERR_INVALID, "smvsb_cut_depth_maps: arguments");
-        if (opts->n_devices < 1 || !opts->devices)
+    if (n_views < 1 || !w || !h || !depth || !normals || !invproj9
+        || !cam_to_world16 || !KR9 || !t3 || !depth_out || !opts)
+        throw Error(SMVSB_ERR_INVALID, "smvsb_cut_depth_maps: arguments");
+    if (opts->n_devices < 1 || !opts->devices)
+        throw Error(SMVSB_ERR_INVALID,
+            "smvsb_cut_depth_maps: empty device list");
+    for (int i = 0; i < n_views; ++i)
+        if (w[i] < 1 || h[i] < 1 || !depth[i] || !normals[i]
+            || !depth_out[i])
             throw Error(SMVSB_ERR_INVALID,
-                "smvsb_cut_depth_maps: empty device list");
-        for (int i = 0; i < n_views; ++i)
-            if (w[i] < 1 || h[i] < 1 || !depth[i] || !normals[i]
-                || !depth_out[i])
-                throw Error(SMVSB_ERR_INVALID,
-                    "smvsb_cut_depth_maps: view without maps");
-        int count = 0;
-        if (cudaGetDeviceCount(&count) != cudaSuccess || count == 0)
-        {
-            cudaGetLastError();
-            throw Error(SMVSB_ERR_CUDA, "no CUDA device (no CPU fallback)");
-        }
-        std::vector<int> const devs(opts->devices,
-            opts->devices + opts->n_devices);
-        for (int d : devs)
-            if (d < 0 || d >= count)
-                throw Error(SMVSB_ERR_INVALID, "device index out of range");
-        std::lock_guard<std::mutex> guard(g_cut_lock);
-        int caller_dev = 0;
-        CUDA_CHECK(cudaGetDevice(&caller_dev));
-        struct Restore
-        {
-            int d;
-            ~Restore (void) { cudaSetDevice(d); }
-        } restore{ caller_dev };
+                "smvsb_cut_depth_maps: view without maps");
+    std::vector<int> const devs(opts->devices,
+        opts->devices + opts->n_devices);
+    for (int d : devs)
+        check_device(d);
+    std::lock_guard<std::mutex> guard(g_cut_lock);
+    int caller_dev = 0;
+    CUDA_CHECK(cudaGetDevice(&caller_dev));
+    struct Restore
+    {
+        int d;
+        ~Restore (void) { cudaSetDevice(d); }
+    } restore{ caller_dev };
 
-        Scene S;
-        S.n = n_views; S.w = w; S.h = h; S.depth = depth; S.normals = normals;
-        S.invproj9 = invproj9; S.ctw16 = cam_to_world16; S.KR9 = KR9;
-        S.t3 = t3; S.out = depth_out;
-        S.nwords = (n_views + 31) / 32;
-        S.max_pix = 0;
-        size_t max_target = 0;
-        for (int i = 0; i < n_views; ++i)
-        {
-            S.max_pix = std::max(S.max_pix, S.pix(i));
-            max_target = std::max(max_target, S.target_bytes(i));
-        }
-        int const n_workers = static_cast<int>(devs.size());
-        S.group_cap = (n_views + n_workers - 1) / n_workers;
-        size_t const least = S.fixed_bytes() + max_target
-            + (n_views > 1 ? S.slot_bytes() : 0);
+    Scene S;
+    S.n = n_views; S.w = w; S.h = h; S.depth = depth; S.normals = normals;
+    S.invproj9 = invproj9; S.ctw16 = cam_to_world16; S.KR9 = KR9;
+    S.t3 = t3; S.out = depth_out;
+    S.nwords = (n_views + 31) / 32;
+    S.max_pix = 0;
+    size_t max_target = 0;
+    for (int i = 0; i < n_views; ++i)
+    {
+        S.max_pix = std::max(S.max_pix, S.pix(i));
+        max_target = std::max(max_target, S.target_bytes(i));
+    }
+    int const n_workers = static_cast<int>(devs.size());
+    S.group_cap = (n_views + n_workers - 1) / n_workers;
+    size_t const least = S.fixed_bytes() + max_target
+        + (n_views > 1 ? S.slot_bytes() : 0);
 
-        /* budget per worker: the device's cap (or its free memory less a
-         * margin) split among the workers on it */
-        std::vector<size_t> budget(n_workers);
-        for (int k = 0; k < n_workers; ++k)
+    /* budget per worker: the device's cap (or its free memory less a
+     * margin) split among the workers on it */
+    std::vector<size_t> budget(n_workers);
+    for (int k = 0; k < n_workers; ++k)
+    {
+        int const d = devs[k];
+        int const share = static_cast<int>(std::count(devs.begin(),
+            devs.end(), d));
+        size_t dev_bytes = opts->device_bytes;
+        if (dev_bytes == 0)
         {
-            int const d = devs[k];
-            int const share = static_cast<int>(std::count(devs.begin(),
-                devs.end(), d));
-            size_t dev_bytes = opts->device_bytes;
-            if (dev_bytes == 0)
-            {
-                CUDA_CHECK(cudaSetDevice(d));
-                size_t free_b = 0, total_b = 0;
-                CUDA_CHECK(cudaMemGetInfo(&free_b, &total_b));
-                size_t const margin = std::max<size_t>(size_t(256) << 20,
-                    total_b / 32);
-                dev_bytes = free_b > margin ? free_b - margin : 0;
-            }
-            budget[k] = dev_bytes / share;
-            if (budget[k] < least)
-                throw Error(opts->device_bytes ? SMVSB_ERR_INVALID
-                    : SMVSB_ERR_ALLOC, "smvsb_cut_depth_maps: "
-                    + std::to_string(budget[k]) + " bytes per worker on "
-                    "device " + std::to_string(d) + " do not hold the "
-                    "largest target view and one source view ("
-                    + std::to_string(least) + " bytes)");
+            CUDA_CHECK(cudaSetDevice(d));
+            size_t free_b = 0, total_b = 0;
+            CUDA_CHECK(cudaMemGetInfo(&free_b, &total_b));
+            size_t const margin = std::max<size_t>(size_t(256) << 20,
+                total_b / 32);
+            dev_bytes = free_b > margin ? free_b - margin : 0;
         }
+        budget[k] = dev_bytes / share;
+        if (budget[k] < least)
+            throw Error(opts->device_bytes ? SMVSB_ERR_INVALID
+                : SMVSB_ERR_ALLOC, "smvsb_cut_depth_maps: "
+                + std::to_string(budget[k]) + " bytes per worker on "
+                "device " + std::to_string(d) + " do not hold the "
+                "largest target view and one source view ("
+                + std::to_string(least) + " bytes)");
+    }
 
-        std::vector<WorkerStats> ws(n_workers);
-        std::vector<std::thread> threads;
+    /* A worker reports through Scene::fail: nothing may leave a thread. The
+     * workers are joined at the end of the block, also when a later one
+     * could not be started. */
+    struct Threads : std::vector<std::thread>
+    {
+        ~Threads (void) { for (std::thread& t : *this) t.join(); }
+    };
+    std::vector<WorkerStats> ws(n_workers);
+    {
+        Threads threads;
         for (int k = 0; k < n_workers; ++k)
             threads.emplace_back([&S, &ws, &devs, &budget, k] {
                 try
@@ -1049,32 +1044,24 @@ cut_depth_maps_multi (smvsb_cut_options const* opts, int n_views,
                     S.fail(Error(SMVSB_ERR_INVALID, e.what()));
                 }
             });
-        for (std::thread& t : threads)
-            t.join();
-        if (S.err_code != SMVSB_OK)
-            throw Error(S.err_code, S.err_msg);
-        if (stats)
-        {
-            smvsb_cut_stats out = {};
-            for (WorkerStats const& s : ws)
-            {
-                out.reference_pairs += s.valid
-                    * static_cast<uint64_t>(n_views - 1);
-                out.evaluated_pairs += s.pairs;
-                out.bytes_uploaded += s.bytes;
-                out.target_groups += s.groups;
-                out.source_chunks += s.chunks;
-                out.ms_device = std::max(out.ms_device, s.ms);
-            }
-            *stats = out;
-        }
     }
-    catch (Error const& e)
+    if (S.err_code != SMVSB_OK)
+        throw Error(S.err_code, S.err_msg);
+    if (stats)
     {
-        g_cut_error = e.msg;
-        rc = e.code;
+        smvsb_cut_stats out = {};
+        for (WorkerStats const& s : ws)
+        {
+            out.reference_pairs += s.valid
+                * static_cast<uint64_t>(n_views - 1);
+            out.evaluated_pairs += s.pairs;
+            out.bytes_uploaded += s.bytes;
+            out.target_groups += s.groups;
+            out.source_chunks += s.chunks;
+            out.ms_device = std::max(out.ms_device, s.ms);
+        }
+        *stats = out;
     }
-    return rc;
 }
 
 } /* namespace smvsb */

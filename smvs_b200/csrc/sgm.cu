@@ -747,8 +747,6 @@ run_paths_wta (int w, int h, unsigned P1, unsigned P2, uint8_t const* cost,
     CUDA_CHECK(cudaGetLastError());
 }
 
-thread_local std::string g_sgm_error;
-
 /*
  * SGMStereo::reconstruct's consistency check (lib/sgm_stereo.cc:64-91): every
  * main-view depth is reprojected into the neighbour (Correspondence::update /
@@ -833,6 +831,7 @@ struct SgmWorkspace
 {
     std::mutex lock;
     bool ready = false;
+    int device = 0;
     cudaStream_t st = nullptr;
     cudaEvent_t ev[8] = {};
     DevBuf<uint8_t> d_main, d_neigh, d_cost, d_D, d_warp;
@@ -861,28 +860,36 @@ check_sgm_args (int w, int h, int nw, int nh, void const* a, void const* b,
             "smvsb_sgm: need penalty1 <= penalty2 <= 255");
 }
 
+/* The start of sgm_run and sgm_reconstruct: the workspace of `device`, held
+ * by `hold` for the call, its stream ready and the two byte images on their
+ * way to the device. */
 SgmWorkspace&
-workspace_for (int device)
+open_workspace (std::unique_lock<std::mutex>& hold, int device, int w, int h,
+    uint8_t const* main_lum, int nw, int nh, uint8_t const* neigh_lum)
 {
-    int count = 0;
-    if (cudaGetDeviceCount(&count) != cudaSuccess || count == 0)
-        throw Error(SMVSB_ERR_CUDA, "no CUDA device (no CPU fallback)");
-    if (device < 0 || device >= count || device >= SMVSB_MAX_DEVICES)
+    check_device(device);
+    if (device >= SMVSB_MAX_DEVICES)
         throw Error(SMVSB_ERR_INVALID, "device index out of range");
-    return g_sgm_ws[device];
-}
-
-void
-prepare_workspace (SgmWorkspace& ws, int device)
-{
+    SgmWorkspace& ws = g_sgm_ws[device];
+    hold = std::unique_lock<std::mutex>(ws.lock);
     CUDA_CHECK(cudaSetDevice(device));
     if (!ws.ready)
     {
         CUDA_CHECK(cudaStreamCreateWithFlags(&ws.st, cudaStreamNonBlocking));
         for (int i = 0; i < 8; ++i)
             CUDA_CHECK(cudaEventCreate(&ws.ev[i]));
+        ws.device = device;
         ws.ready = true;
     }
+    size_t const npix = static_cast<size_t>(w) * h;
+    size_t const nnpix = static_cast<size_t>(nw) * nh;
+    ws.d_main.reserve(npix);
+    ws.d_neigh.reserve(nnpix);
+    CUDA_CHECK(cudaMemcpyAsync(ws.d_main.p, main_lum, npix,
+        cudaMemcpyHostToDevice, ws.st));
+    CUDA_CHECK(cudaMemcpyAsync(ws.d_neigh.p, neigh_lum, nnpix,
+        cudaMemcpyHostToDevice, ws.st));
+    return ws;
 }
 
 /* create_cost_volume + aggregate_sgm_costs + depth_from_sgm_volume for the
@@ -961,85 +968,66 @@ sgm_pair (SgmWorkspace& ws, int w, int h, uint8_t const* main_dev, int nw,
     case 128: run_paths_wta<128>(w, h, P1, P2, ws.d_cost.p, ws.d_D.p, main_dev, depths_dev, S_dev, out_dev, ws.ev[e0 + 2], st); break;
     default: run_paths_wta<256>(w, h, P1, P2, ws.d_cost.p, ws.d_D.p, main_dev, depths_dev, S_dev, out_dev, ws.ev[e0 + 2], st); break;
     }
+    /* u8_to_float, warp volume, cost bits, paths, sum + WTA */
+    count_device_launches(ws.device, 5);
     CUDA_CHECK(cudaEventRecord(ws.ev[e0 + 3], st));
 }
 
 } /* namespace */
 
-std::string const&
-sgm_last_error (void)
-{
-    return g_sgm_error;
-}
-
-int
+void
 sgm_run (int device, int w, int h, uint8_t const* main_lum, int nw, int nh,
     uint8_t const* neigh_lum, float const* M, float const* t,
     float min_depth, float max_depth, int num_steps, uint16_t penalty1,
     uint16_t penalty2, float* depth_out, uint16_t* cost_out,
     uint16_t* sgm_out, double* ms_out)
 {
-    int rc = SMVSB_OK;
-    try
+    check_sgm_args(w, h, nw, nh, main_lum, neigh_lum, M, t, depth_out,
+        num_steps, penalty1, penalty2);
+    std::unique_lock<std::mutex> hold;
+    SgmWorkspace& ws = open_workspace(hold, device, w, h, main_lum, nw, nh,
+        neigh_lum);
+    cudaStream_t st = ws.st;
+    size_t const npix = static_cast<size_t>(w) * h;
+    size_t const nvox = npix * num_steps;
+    ws.d_out.reserve(npix);
+    if (cost_out)
+        ws.d_S.reserve(nvox);
+    sgm_pair(ws, w, h, ws.d_main.p, nw, nh, ws.d_neigh.p, M, t, min_depth,
+        max_depth, num_steps, penalty1, penalty2, sgm_out != nullptr,
+        ws.d_out.p, 0);
+    CUDA_CHECK(cudaMemcpyAsync(depth_out, ws.d_out.p, npix * sizeof(float),
+        cudaMemcpyDeviceToHost, st));
+    if (sgm_out)
+        CUDA_CHECK(cudaMemcpyAsync(sgm_out, ws.d_S.p,
+            nvox * sizeof(uint16_t), cudaMemcpyDeviceToHost, st));
+    CUDA_CHECK(cudaStreamSynchronize(st));
+    if (cost_out)
     {
-        check_sgm_args(w, h, nw, nh, main_lum, neigh_lum, M, t, depth_out,
-            num_steps, penalty1, penalty2);
-        SgmWorkspace& ws = workspace_for(device);
-        std::lock_guard<std::mutex> guard(ws.lock);
-        prepare_workspace(ws, device);
-        cudaStream_t st = ws.st;
-        size_t const npix = static_cast<size_t>(w) * h;
-        size_t const nvox = npix * num_steps;
-        ws.d_main.reserve(npix);
-        ws.d_neigh.reserve(static_cast<size_t>(nw) * nh);
-        ws.d_out.reserve(npix);
-        if (cost_out)
-            ws.d_S.reserve(nvox);
-        CUDA_CHECK(cudaMemcpyAsync(ws.d_main.p, main_lum, npix,
-            cudaMemcpyHostToDevice, st));
-        CUDA_CHECK(cudaMemcpyAsync(ws.d_neigh.p, neigh_lum,
-            static_cast<size_t>(nw) * nh, cudaMemcpyHostToDevice, st));
-        sgm_pair(ws, w, h, ws.d_main.p, nw, nh, ws.d_neigh.p, M, t, min_depth,
-            max_depth, num_steps, penalty1, penalty2, sgm_out != nullptr,
-            ws.d_out.p, 0);
-        CUDA_CHECK(cudaMemcpyAsync(depth_out, ws.d_out.p, npix * sizeof(float),
-            cudaMemcpyDeviceToHost, st));
-        if (sgm_out)
-            CUDA_CHECK(cudaMemcpyAsync(sgm_out, ws.d_S.p,
-                nvox * sizeof(uint16_t), cudaMemcpyDeviceToHost, st));
+        /* widen through the (now free) S buffer */
+        u8_to_u16_kernel<<<static_cast<unsigned>((nvox + 255) / 256), 256,
+            0, st>>>(nvox, ws.d_cost.p, ws.d_S.p);
+        CUDA_CHECK(cudaGetLastError());
+        count_device_launches(device, 1);
+        CUDA_CHECK(cudaMemcpyAsync(cost_out, ws.d_S.p,
+            nvox * sizeof(uint16_t), cudaMemcpyDeviceToHost, st));
         CUDA_CHECK(cudaStreamSynchronize(st));
-        if (cost_out)
-        {
-            /* widen through the (now free) S buffer */
-            u8_to_u16_kernel<<<static_cast<unsigned>((nvox + 255) / 256), 256,
-                0, st>>>(nvox, ws.d_cost.p, ws.d_S.p);
-            CUDA_CHECK(cudaGetLastError());
-            CUDA_CHECK(cudaMemcpyAsync(cost_out, ws.d_S.p,
-                nvox * sizeof(uint16_t), cudaMemcpyDeviceToHost, st));
-            CUDA_CHECK(cudaStreamSynchronize(st));
-        }
-        if (ms_out)
-        {
-            float ms;
-            for (int i = 0; i < 3; ++i)
-            {
-                CUDA_CHECK(cudaEventElapsedTime(&ms, ws.ev[i], ws.ev[i + 1]));
-                ms_out[i] = ms;
-            }
-        }
     }
-    catch (Error const& e)
+    if (ms_out)
     {
-        g_sgm_error = e.msg;
-        rc = e.code;
+        float ms;
+        for (int i = 0; i < 3; ++i)
+        {
+            CUDA_CHECK(cudaEventElapsedTime(&ms, ws.ev[i], ws.ev[i + 1]));
+            ms_out[i] = ms;
+        }
     }
-    return rc;
 }
 
 /* SGMStereo::reconstruct (lib/sgm_stereo.cc:45-96) for an image pair at SGM
  * working resolution, optionally followed by the merge of
  * app/smvsrecon.cc:362-377 with an earlier result. */
-int
+void
 sgm_reconstruct (int device, int w, int h, uint8_t const* main_lum, int nw,
     int nh, uint8_t const* neigh_lum, float const* M_mn, float const* t_mn,
     float const* M_nm, float const* t_nm, float const* depth_range_main,
@@ -1047,77 +1035,61 @@ sgm_reconstruct (int device, int w, int h, uint8_t const* main_lum, int nw,
     uint16_t penalty2, float const* merge_with, float* depth_out,
     double* ms_out)
 {
-    int rc = SMVSB_OK;
-    try
+    check_sgm_args(w, h, nw, nh, main_lum, neigh_lum, M_mn, t_mn, depth_out,
+        num_steps, penalty1, penalty2);
+    if (!(nw > 9 && nh > 7 && M_nm && t_nm && depth_range_main
+        && depth_range_neigh))
+        throw Error(SMVSB_ERR_INVALID, "smvsb_sgm_reconstruct: bad arguments");
+    std::unique_lock<std::mutex> hold;
+    SgmWorkspace& ws = open_workspace(hold, device, w, h, main_lum, nw, nh,
+        neigh_lum);
+    cudaStream_t st = ws.st;
+    size_t const npix = static_cast<size_t>(w) * h;
+    ws.d_out.reserve(npix);
+    ws.d_out2.reserve(static_cast<size_t>(nw) * nh);
+    if (merge_with != nullptr)
     {
-        check_sgm_args(w, h, nw, nh, main_lum, neigh_lum, M_mn, t_mn,
-            depth_out, num_steps, penalty1, penalty2);
-        if (!(nw > 9 && nh > 7 && M_nm && t_nm && depth_range_main
-            && depth_range_neigh))
-            throw Error(SMVSB_ERR_INVALID,
-                "smvsb_sgm_reconstruct: bad arguments");
-        SgmWorkspace& ws = workspace_for(device);
-        std::lock_guard<std::mutex> guard(ws.lock);
-        prepare_workspace(ws, device);
-        cudaStream_t st = ws.st;
-        size_t const npix = static_cast<size_t>(w) * h;
-        size_t const nnpix = static_cast<size_t>(nw) * nh;
-        ws.d_main.reserve(npix);
-        ws.d_neigh.reserve(nnpix);
-        ws.d_out.reserve(npix);
-        ws.d_out2.reserve(nnpix);
-        CUDA_CHECK(cudaMemcpyAsync(ws.d_main.p, main_lum, npix,
-            cudaMemcpyHostToDevice, st));
-        CUDA_CHECK(cudaMemcpyAsync(ws.d_neigh.p, neigh_lum, nnpix,
-            cudaMemcpyHostToDevice, st));
-        if (merge_with != nullptr)
-        {
-            ws.d_prev.reserve(npix);
-            CUDA_CHECK(cudaMemcpyAsync(ws.d_prev.p, merge_with,
-                npix * sizeof(float), cudaMemcpyHostToDevice, st));
-        }
-        /* sgm1: main against neighbour; sgm2: the roles swapped (:56-62) */
-        sgm_pair(ws, w, h, ws.d_main.p, nw, nh, ws.d_neigh.p, M_mn, t_mn,
-            depth_range_main[0], depth_range_main[1], num_steps, penalty1,
-            penalty2, false, ws.d_out.p, 0);
-        sgm_pair(ws, nw, nh, ws.d_neigh.p, w, h, ws.d_main.p, M_nm, t_nm,
-            depth_range_neigh[0], depth_range_neigh[1], num_steps, penalty1,
-            penalty2, false, ws.d_out2.p, 4);
+        ws.d_prev.reserve(npix);
+        CUDA_CHECK(cudaMemcpyAsync(ws.d_prev.p, merge_with,
+            npix * sizeof(float), cudaMemcpyHostToDevice, st));
+    }
+    /* sgm1: main against neighbour; sgm2: the roles swapped (:56-62) */
+    sgm_pair(ws, w, h, ws.d_main.p, nw, nh, ws.d_neigh.p, M_mn, t_mn,
+        depth_range_main[0], depth_range_main[1], num_steps, penalty1,
+        penalty2, false, ws.d_out.p, 0);
+    sgm_pair(ws, nw, nh, ws.d_neigh.p, w, h, ws.d_main.p, M_nm, t_nm,
+        depth_range_neigh[0], depth_range_neigh[1], num_steps, penalty1,
+        penalty2, false, ws.d_out2.p, 4);
 
-        ConsistencyParams cp;
-        cp.w = w; cp.h = h; cp.nw = nw; cp.nh = nh;
-        cp.cut = static_cast<int>(0.03 * std::max(nw, nh));
-        for (int i = 0; i < 9; ++i) cp.M[i] = M_mn[i];
-        for (int i = 0; i < 3; ++i) cp.t[i] = t_mn[i];
-        dim3 const block(32, 8);
-        dim3 const grid((w + 31) / 32, (h + 7) / 8);
-        sgm_consistency_kernel<<<grid, block, 0, st>>>(cp, ws.d_out.p,
-            ws.d_out2.p);
-        CUDA_CHECK(cudaGetLastError());
-        if (merge_with != nullptr)
-        {
-            sgm_merge_kernel<<<static_cast<unsigned>((npix + 255) / 256), 256,
-                0, st>>>(npix, ws.d_prev.p, ws.d_out.p);
-            CUDA_CHECK(cudaGetLastError());
-        }
-        CUDA_CHECK(cudaMemcpyAsync(depth_out, ws.d_out.p, npix * sizeof(float),
-            cudaMemcpyDeviceToHost, st));
-        CUDA_CHECK(cudaStreamSynchronize(st));
-        if (ms_out)
-        {
-            float ms;
-            CUDA_CHECK(cudaEventElapsedTime(&ms, ws.ev[0], ws.ev[3]));
-            ms_out[0] = ms;
-            CUDA_CHECK(cudaEventElapsedTime(&ms, ws.ev[4], ws.ev[7]));
-            ms_out[1] = ms;
-        }
-    }
-    catch (Error const& e)
+    ConsistencyParams cp;
+    cp.w = w; cp.h = h; cp.nw = nw; cp.nh = nh;
+    cp.cut = static_cast<int>(0.03 * std::max(nw, nh));
+    for (int i = 0; i < 9; ++i) cp.M[i] = M_mn[i];
+    for (int i = 0; i < 3; ++i) cp.t[i] = t_mn[i];
+    dim3 const block(32, 8);
+    dim3 const grid((w + 31) / 32, (h + 7) / 8);
+    sgm_consistency_kernel<<<grid, block, 0, st>>>(cp, ws.d_out.p,
+        ws.d_out2.p);
+    CUDA_CHECK(cudaGetLastError());
+    count_device_launches(device, 1);
+    if (merge_with != nullptr)
     {
-        g_sgm_error = e.msg;
-        rc = e.code;
+        sgm_merge_kernel<<<static_cast<unsigned>((npix + 255) / 256), 256,
+            0, st>>>(npix, ws.d_prev.p, ws.d_out.p);
+        CUDA_CHECK(cudaGetLastError());
+        count_device_launches(device, 1);
     }
-    return rc;
+    CUDA_CHECK(cudaMemcpyAsync(depth_out, ws.d_out.p, npix * sizeof(float),
+        cudaMemcpyDeviceToHost, st));
+    CUDA_CHECK(cudaStreamSynchronize(st));
+    if (ms_out)
+    {
+        float ms;
+        CUDA_CHECK(cudaEventElapsedTime(&ms, ws.ev[0], ws.ev[3]));
+        ms_out[0] = ms;
+        CUDA_CHECK(cudaEventElapsedTime(&ms, ws.ev[4], ws.ev[7]));
+        ms_out[1] = ms;
+    }
 }
 
 } /* namespace smvsb */

@@ -15,8 +15,6 @@
  *   K5  light_partials_kernel  LightOptimizer::fit_lighting_to_image sums
  *                        (lib/light_optimizer.cc:22-55)
  */
-#include <cstring>
-
 #include "gn_math.cuh"
 #include "patch_eval.cuh"
 
@@ -383,7 +381,7 @@ update_enqueue (smvsb_ctx* c, double thresh, bool full_opt)
         c->upd_partials.p, c->upd_result.p);
     CUDA_CHECK(cudaGetLastError());
     smvsb::count_launches(c, 4);
-    CUDA_CHECK(cudaMemcpyAsync(c->h_scalars + 12, c->upd_result.p,
+    CUDA_CHECK(cudaMemcpyAsync(c->pinned->update, c->upd_result.p,
         3 * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
 }
 
@@ -391,7 +389,7 @@ update_enqueue (smvsb_ctx* c, double thresh, bool full_opt)
 void
 update_collect (smvsb_ctx* c, uint64_t* n_active, double* mean_shift)
 {
-    double const* res = c->h_scalars + 12;
+    double const* res = c->pinned->update;
     if (n_active) *n_active = static_cast<uint64_t>(res[2]);
     if (mean_shift) *mean_shift = res[0] / res[1];
 }
@@ -416,16 +414,14 @@ count_processed_enqueue (smvsb_ctx* c)
         c->stream>>>(sf, c->counters.p);
     smvsb::count_launches(c, 1);
     CUDA_CHECK(cudaGetLastError());
-    CUDA_CHECK(cudaMemcpyAsync(c->h_scalars + 16, c->counters.p,
+    CUDA_CHECK(cudaMemcpyAsync(&c->pinned->processed, c->counters.p,
         sizeof(unsigned long long), cudaMemcpyDeviceToHost, c->stream));
 }
 
 unsigned long long
 count_processed_collect (smvsb_ctx* c)
 {
-    unsigned long long n;
-    memcpy(&n, c->h_scalars + 16, sizeof(n));
-    return n;
+    return c->pinned->processed;
 }
 
 void

@@ -123,6 +123,34 @@ def test_golden_sgm_bit_exact():
     assert np.array_equal(r["depth"], G["depth"])
 
 
+def test_sgm_device_launch_counts():
+    """smvsb_device_launch_count grows by the kernels an SGM call launches: a
+    pair is u8_to_float, warp volume, cost bits, paths and sum + WTA; the cost
+    volume's widening adds one; reconstruct is two pairs and the consistency
+    check, plus the merge."""
+    G = load("sgm.npz")
+    L = api.lib()
+    dmin, dmax, D = float(G["min_depth"]), float(G["max_depth"]), int(G["D"])
+
+    def launched(fn):
+        before = L.smvsb_device_launch_count(0)
+        fn()
+        return L.smvsb_device_launch_count(0) - before
+
+    def sgm(volumes):
+        api.sgm(G["main"], G["neigh"], G["M"], G["t"], dmin, dmax, D, volumes=volumes)
+
+    def rec(merge_with):
+        api.sgm_reconstruct(G["main"], G["neigh"], G["M"], G["t"], G["M"], G["t"],
+                            (dmin, dmax), (dmin, dmax), D, merge_with=merge_with)
+
+    prev = np.zeros(G["main"].shape, np.float32)
+    assert launched(lambda: sgm(False)) == 5
+    assert launched(lambda: sgm(True)) == 6
+    assert launched(lambda: rec(None)) == 11
+    assert launched(lambda: rec(prev)) == 12
+
+
 @pytest.mark.parametrize("w,h", [(333, 207), (352, 207)])
 def test_device_set_scale_bitwise(w, h):
     """smvsb_set_views_u8 (StereoView::set_scale on the device) against the
