@@ -14,28 +14,6 @@
 #include "common.cuh"
 
 namespace smvsb {
-void fill_basis_table (std::vector<double>& tab, int ps, int step);
-void device_set_scale (smvsb_ctx* c, uint8_t const* img_dev, int w, int h,
-    int scale, float* tmp_a, float* tmp_b, int mode, float* out_dev);
-void device_shading_inputs (smvsb_ctx* c, uint8_t const* img_dev, int w, int h,
-    float* shading_dev, float* shading_grad_dev);
-void device_set_scale_float (smvsb_ctx* c, float const* img_dev, int w, int h,
-    int scale, float* tmp_a, float* tmp_b, float* out_dev);
-void device_set_scale_rgb (smvsb_ctx* c, float const* img_dev, int w, int h,
-    int scale, float* tmp_a, float* tmp_b, int mode, float* out_dev,
-    float* blur_out);
-void device_bilateral_filter (smvsb_ctx* c, float const* ci_dev, int w, int h,
-    int channels, float const* dm_dev, int dm_w, int dm_h, float sigma,
-    int kernel_size, float* out_dev);
-float host_expf_like_glibc (float x);
-void device_byte_to_float (smvsb_ctx* c, uint8_t const* img_dev, size_t n,
-    float* out_dev);
-void device_unpack_texels (smvsb_ctx* c, float const* texels, int n,
-    float* grad, float* hess);
-double measure_fp64_peak (int device);
-}
-
-namespace smvsb {
 std::atomic<uint64_t> g_launches(0);
 std::atomic<uint64_t> g_device_launches[SMVSB_MAX_DEVICES];
 }
@@ -284,6 +262,24 @@ set_neighbour_tables (smvsb_ctx* c, int n_sub, int const* sub_w,
     upload(c, c->Mt, mt.data(), mt.size());
 }
 
+/* The three-channel images of the main view and of each neighbour, at the
+ * sizes the context holds, and the device array of the neighbours' image
+ * pointers that the NCC filter reads. */
+void
+upload_color_images (smvsb_ctx* c, float const* main_rgb,
+    float const* const* sub_rgb)
+{
+    upload(c, c->color_main, main_rgb, static_cast<size_t>(c->w) * c->h * 3);
+    std::vector<float const*> ptrs(c->n_sub);
+    for (int k = 0; k < c->n_sub; ++k)
+    {
+        upload(c, c->color_subs[k], sub_rgb[k],
+            static_cast<size_t>(c->subs[k].w) * c->subs[k].h * 3);
+        ptrs[k] = c->color_subs[k].p;
+    }
+    upload(c, c->color_ptrs, ptrs.data(), ptrs.size());
+}
+
 void
 ensure_system_buffers (smvsb_ctx* c)
 {
@@ -429,29 +425,24 @@ surface_subdivide_device (smvsb_ctx* c)
 void
 views_from_resident (smvsb_ctx* c, int scale, bool colour)
 {
+    smvsb::DevImage::Kind const kind = colour ? smvsb::DevImage::RGB_F32
+        : smvsb::DevImage::U8;
     size_t max_pix = static_cast<size_t>(c->w) * c->h;
     for (int k = 0; k < c->n_sub; ++k)
         max_pix = std::max(max_pix, static_cast<size_t>(c->subs[k].w)
             * c->subs[k].h);
-    c->stage_a.reserve(max_pix * (colour ? 3 : 1));
-    c->stage_b.reserve(max_pix);
+    smvsb::reserve_set_scale_scratch(c, kind, max_pix);
     c->main_grad.reserve(static_cast<size_t>(c->w) * c->h * 2);
-    if (colour)
-        smvsb::device_set_scale_rgb(c, c->color_main.p, c->w, c->h, scale,
-            c->stage_a.p, c->stage_b.p, 0, c->main_grad.p, nullptr);
-    else
-        smvsb::device_set_scale(c, c->u8_main.p, c->w, c->h, scale,
-            c->stage_a.p, c->stage_b.p, 0, c->main_grad.p);
+    smvsb::device_set_scale(c, { kind, colour
+        ? static_cast<void const*>(c->color_main.p) : c->u8_main.p, c->w,
+        c->h }, scale, 0, c->main_grad.p, nullptr);
     for (int k = 0; k < c->n_sub; ++k)
     {
         smvsb::SubViewDev& sv = c->subs[k];
         sv.texels.reserve(static_cast<size_t>(sv.w) * sv.h * SMVSB_NB_STRIDE);
-        if (colour)
-            smvsb::device_set_scale_rgb(c, c->color_subs[k].p, sv.w, sv.h,
-                scale, c->stage_a.p, c->stage_b.p, 1, sv.texels.p, nullptr);
-        else
-            smvsb::device_set_scale(c, c->u8_subs[k].p, sv.w, sv.h, scale,
-                c->stage_a.p, c->stage_b.p, 1, sv.texels.p);
+        smvsb::device_set_scale(c, { kind, colour
+            ? static_cast<void const*>(c->color_subs[k].p) : c->u8_subs[k].p,
+            sv.w, sv.h }, scale, 1, sv.texels.p, nullptr);
     }
     c->have_system = false;
 }
@@ -659,8 +650,7 @@ smvsb_set_views_u8 (smvsb_ctx* ctx, int scale, int w, int h, double flen_px,
         set_neighbour_tables(c, n_sub, sub_w, sub_h, Mi, ti);
         c->stage_u8.reserve(max_pix);
         c->stage_u8b.reserve(max_pix);
-        c->stage_a.reserve(max_pix);
-        c->stage_b.reserve(max_pix);
+        smvsb::reserve_set_scale_scratch(c, smvsb::DevImage::U8, max_pix);
         size_t const npix = static_cast<size_t>(w) * h;
         c->main_grad.reserve(npix * 2);
         /* Image k travels on the copy stream into staging buffer k mod 2
@@ -692,8 +682,8 @@ smvsb_set_views_u8 (smvsb_ctx* ctx, int scale, int w, int h, double flen_px,
             stage_image(1, sub_img[0], static_cast<size_t>(sub_w[0]) * sub_h[0]);
         {
             uint8_t const* src = acquire(0);
-            smvsb::device_set_scale(c, src, w, h, scale, c->stage_a.p,
-                c->stage_b.p, 0, c->main_grad.p);
+            smvsb::device_set_scale(c, { smvsb::DevImage::U8, src, w, h },
+                scale, 0, c->main_grad.p, nullptr);
             c->have_shading = (with_shading != 0);
             if (c->have_shading)
             {
@@ -711,8 +701,8 @@ smvsb_set_views_u8 (smvsb_ctx* ctx, int scale, int w, int h, double flen_px,
                 stage_image(k + 2, sub_img[k + 1],
                     static_cast<size_t>(sub_w[k + 1]) * sub_h[k + 1]);
             uint8_t const* src = acquire(k + 1);
-            smvsb::device_set_scale(c, src, sv.w, sv.h, scale,
-                c->stage_a.p, c->stage_b.p, 1, sv.texels.p);
+            smvsb::device_set_scale(c, { smvsb::DevImage::U8, src, sv.w,
+                sv.h }, scale, 1, sv.texels.p, nullptr);
             release(k + 1);
         }
         CUDA_CHECK(cudaStreamSynchronize(c->stream));
@@ -765,27 +755,19 @@ smvsb_view_set_scale_c (smvsb_ctx* ctx, int w, int h, int channels,
             "scale out of range");
         size_t const n = static_cast<size_t>(w) * h;
         size_t const nc = n * channels;
-        c->stage_a.reserve(nc);
-        c->stage_b.reserve(n);
         c->view_in.reserve(nc);
         c->view_texels.reserve(n * SMVSB_NB_STRIDE);
         c->view_out.reserve(n * 5);
         CUDA_CHECK(cudaMemcpyAsync(c->view_in.p, image, nc * sizeof(float),
             cudaMemcpyHostToDevice, c->stream));
-        float const* blurred = c->stage_b.p;
-        if (channels == 1)
-            smvsb::device_set_scale_float(c, c->view_in.p, w, h, scale,
-                c->stage_a.p, c->stage_b.p, c->view_texels.p);
-        else
-        {
-            /* the blurred colour image overwrites the input copy */
-            smvsb::device_set_scale_rgb(c, c->view_in.p, w, h, scale,
-                c->stage_a.p, c->stage_b.p, 1, c->view_texels.p,
-                (scaleimage != nullptr) ? c->view_in.p : nullptr);
-            blurred = c->view_in.p;
-        }
+        /* the blurred image passes through view_out before the gradient and
+         * Hessian are unpacked into it */
+        smvsb::device_set_scale(c, { channels == 1 ? smvsb::DevImage::F32
+            : smvsb::DevImage::RGB_F32, c->view_in.p, w, h }, scale, 1,
+            c->view_texels.p, (scaleimage != nullptr) ? c->view_out.p
+            : nullptr);
         if (scaleimage != nullptr)
-            CUDA_CHECK(cudaMemcpyAsync(scaleimage, blurred,
+            CUDA_CHECK(cudaMemcpyAsync(scaleimage, c->view_out.p,
                 nc * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
         if (grad != nullptr || hess != nullptr)
         {
@@ -1333,28 +1315,18 @@ optimize_resident (smvsb_ctx* ctx, int w, int h, double flen_px,
         set_neighbour_tables(c, n_sub, sub_w, sub_h, Mi, ti);
         size_t const npix = static_cast<size_t>(w) * h;
         if (colour)
-            upload(c, c->color_main, static_cast<float const*>(main_img),
-                npix * 3);
-        else
-            upload(c, c->u8_main, static_cast<uint8_t const*>(main_img), npix);
-        std::vector<float const*> colour_ptrs(n_sub, nullptr);
-        for (int k = 0; k < n_sub; ++k)
         {
-            size_t const n = static_cast<size_t>(sub_w[k]) * sub_h[k];
-            if (colour)
-            {
-                upload(c, c->color_subs[k],
-                    static_cast<float const*>(sub_img[k]), n * 3);
-                colour_ptrs[k] = c->color_subs[k].p;
-            }
-            else
-                upload(c, c->u8_subs[k],
-                    static_cast<uint8_t const*>(sub_img[k]), n);
-        }
-        if (colour)
-        {
-            upload(c, c->color_ptrs, colour_ptrs.data(), colour_ptrs.size());
+            upload_color_images(c, static_cast<float const*>(main_img),
+                reinterpret_cast<float const* const*>(sub_img));
             c->have_color = true;
+        }
+        else
+        {
+            upload(c, c->u8_main, static_cast<uint8_t const*>(main_img), npix);
+            for (int k = 0; k < n_sub; ++k)
+                upload(c, c->u8_subs[k],
+                    static_cast<uint8_t const*>(sub_img[k]),
+                    static_cast<size_t>(sub_w[k]) * sub_h[k]);
         }
         c->have_shading = (shading != nullptr);
         if (c->have_shading)
@@ -1585,26 +1557,10 @@ smvsb_set_color_images (smvsb_ctx* ctx, const float* main_rgb, int n_sub,
         require(main_rgb != nullptr && sub_rgb != nullptr
             && n_sub == ctx->n_sub, SMVSB_ERR_INVALID,
             "colour images: one per view of the context");
-        size_t const npix = static_cast<size_t>(ctx->w) * ctx->h;
-        ctx->color_main.reserve(npix * 3);
-        CUDA_CHECK(cudaMemcpyAsync(ctx->color_main.p, main_rgb,
-            npix * 3 * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
-        std::vector<float const*> ptrs(n_sub);
         for (int k = 0; k < n_sub; ++k)
-        {
             require(sub_rgb[k] != nullptr, SMVSB_ERR_INVALID,
                 "colour image missing");
-            size_t const n = static_cast<size_t>(ctx->subs[k].w)
-                * ctx->subs[k].h * 3;
-            ctx->color_subs[k].reserve(n);
-            CUDA_CHECK(cudaMemcpyAsync(ctx->color_subs[k].p, sub_rgb[k],
-                n * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
-            ptrs[k] = ctx->color_subs[k].p;
-        }
-        ctx->color_ptrs.reserve(n_sub + 1);
-        CUDA_CHECK(cudaMemcpyAsync(ctx->color_ptrs.p, ptrs.data(),
-            n_sub * sizeof(float const*), cudaMemcpyHostToDevice,
-            ctx->stream));
+        upload_color_images(ctx, main_rgb, sub_rgb);
         CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
         ctx->have_color = true;
     });

@@ -904,54 +904,6 @@ cg_mark_kernel (int npx, int npy, uint8_t const* __restrict__ node_valid,
     }
 }
 
-/* exclusive prefix sum of the per-block row counts, one block */
-__global__ void __launch_bounds__(1024)
-cg_scan_kernel (uint32_t const* __restrict__ block_rows,
-    uint32_t* __restrict__ block_off, int nb)
-{
-    __shared__ uint32_t s_warp[32];
-    __shared__ uint32_t s_carry;
-    if (threadIdx.x == 0)
-        s_carry = 0;
-    __syncthreads();
-    int const lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    for (int base = 0; base < nb; base += 1024)
-    {
-        int const i = base + threadIdx.x;
-        uint32_t const v = (i < nb) ? block_rows[i] : 0;
-        uint32_t inc = v;
-        for (int o = 1; o < 32; o <<= 1)
-        {
-            uint32_t const u = __shfl_up_sync(0xffffffffu, inc, o);
-            if (lane >= o)
-                inc += u;
-        }
-        if (lane == 31)
-            s_warp[warp] = inc;
-        __syncthreads();
-        if (warp == 0)
-        {
-            uint32_t w = s_warp[lane];
-            for (int o = 1; o < 32; o <<= 1)
-            {
-                uint32_t const u = __shfl_up_sync(0xffffffffu, w, o);
-                if (lane >= o)
-                    w += u;
-            }
-            s_warp[lane] = w;
-        }
-        __syncthreads();
-        uint32_t const before = s_carry + (warp > 0 ? s_warp[warp - 1] : 0)
-            + inc - v;
-        if (i < nb)
-            block_off[i] = before;
-        __syncthreads();
-        if (threadIdx.x == 1023)
-            s_carry = before + v;
-        __syncthreads();
-    }
-}
-
 /* rows[]: the nodes with a non-empty row in ascending order -- the solver
  * walks this list, so the work is spread evenly over the CTAs however the
  * active set is scattered over the image */
@@ -998,18 +950,19 @@ mark_system (smvsb_ctx* c)
     int const nb = (c->n_nodes + 255) / 256;
     c->cg_rowmask.reserve(c->n_nodes);
     c->cg_row_list.reserve(c->n_nodes);
-    c->cg_block_rows.reserve(2 * static_cast<size_t>(nb));
+    /* the per-block row counts, then their prefix sum and its total */
+    c->cg_block_rows.reserve(2 * static_cast<size_t>(nb) + 1);
     c->cg_counts.reserve(2);
     CUDA_CHECK(cudaMemsetAsync(c->cg_counts.p, 0,
         2 * sizeof(unsigned long long), c->stream));
     cg_mark_kernel<<<nb, 256, 0, c->stream>>>(c->npx, c->npy,
         c->node_valid.p, c->active.p, c->cg_rowmask.p, c->cg_block_rows.p,
         c->cg_counts.p);
-    cg_scan_kernel<<<1, 1024, 0, c->stream>>>(c->cg_block_rows.p,
-        c->cg_block_rows.p + nb, nb);
+    CUDA_CHECK(cudaGetLastError());
+    launch_exclusive_scan(c, c->cg_block_rows.p, c->cg_block_rows.p + nb, nb);
     cg_list_kernel<<<nb, 256, 0, c->stream>>>(c->n_nodes, c->cg_rowmask.p,
         c->cg_block_rows.p + nb, c->cg_row_list.p);
-    smvsb::count_launches(c, 3);
+    smvsb::count_launches(c, 2);
     CUDA_CHECK(cudaGetLastError());
 }
 

@@ -274,7 +274,36 @@ surface_args (smvsb_ctx* c)
     return s;
 }
 
+/* A view's image on the device as StereoView::set_scale takes it: w*h bytes,
+ * w*h floats, or w*h*3 interleaved floats of a colour view. */
+struct DevImage
+{
+    enum Kind { U8, F32, RGB_F32 } kind;
+    void const* p;
+    int w, h;
+};
+
 /* kernels / launchers implemented in the .cu files */
+void reserve_set_scale_scratch (smvsb_ctx* c, DevImage::Kind kind,
+    size_t pixels);
+/* StereoView::set_scale of one image: blur, then the gradient (mode 0,
+ * float2 per pixel) or the packed neighbour texels (mode 1) into out. The
+ * blurred image (the colour image for RGB_F32) goes to blur_out unless it is
+ * null. */
+void device_set_scale (smvsb_ctx* c, DevImage const& img, int scale, int mode,
+    float* out, float* blur_out);
+void device_shading_inputs (smvsb_ctx* c, uint8_t const* img_dev, int w, int h,
+    float* shading_dev, float* shading_grad_dev);
+void device_bilateral_filter (smvsb_ctx* c, float const* ci_dev, int w, int h,
+    int channels, float const* dm_dev, int dm_w, int dm_h, float sigma,
+    int kernel_size, float* out_dev);
+float host_expf_like_glibc (float x);
+void device_byte_to_float (smvsb_ctx* c, uint8_t const* img_dev, size_t n,
+    float* out_dev);
+void device_unpack_texels (smvsb_ctx* c, float const* texels, int n,
+    float* grad, float* hess);
+void fill_basis_table (std::vector<double>& tab, int ps, int step);
+double measure_fp64_peak (int device);
 void launch_pack_subview (smvsb_ctx* c, float const* grad, float const* hess,
     float* texels, int w, int h);
 void launch_construct (smvsb_ctx* c, bool use_light, double reg,
@@ -299,6 +328,10 @@ uint64_t run_visibility (smvsb_ctx* c, float const* sgm_depth_host);
 uint64_t run_visibility_device (smvsb_ctx* c, bool use_sgm = true);   /* c->sgm_depth already set */
 uint64_t run_visibility_ncc (smvsb_ctx* c);      /* use_sgm = false, colour images set */
 void launch_remove_nodes (smvsb_ctx* c);
+/* off[i] = counts[0] + ... + counts[i - 1] for i = 0 .. n (off[n]: the
+ * total); one block of 1024 threads */
+void launch_exclusive_scan (smvsb_ctx* c, uint32_t const* counts,
+    uint32_t* off, int n);
 void topo_fill_from_depth (smvsb_ctx* c);
 void topo_set_init_depth (smvsb_ctx* c, float const* src_dev);
 void topo_subdivide (smvsb_ctx* c, int* new_npx, int* new_npy, int* new_sx,

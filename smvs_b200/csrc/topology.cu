@@ -43,8 +43,6 @@
 
 namespace smvsb {
 
-void launch_remove_nodes (smvsb_ctx* c);
-
 namespace {
 
 /* One warp per node. Window values (floats) are gathered into shared memory,
@@ -185,26 +183,11 @@ init_nodes_kernel (int npx, int npy, int ps, int sx, int sy, int w, int h,
     }
 }
 
-/* a patch wherever its four nodes exist */
+/* a patch wherever its four nodes exist; counter (unless null) counts the
+ * new patches, as Surface::expand returns them */
 __global__ void
 fill_holes_kernel (int npx, int npy, uint8_t const* __restrict__ node_valid,
-    uint8_t* __restrict__ patch_valid)
-{
-    int const patch = blockIdx.x * blockDim.x + threadIdx.x;
-    if (patch >= npx * npy || patch_valid[patch])
-        return;
-    int const idx = patch % npx, idy = patch / npx;
-    int const n0 = idy * (npx + 1) + idx;
-    if (node_valid[n0] && node_valid[n0 + 1] && node_valid[n0 + npx + 1]
-        && node_valid[n0 + npx + 2])
-        patch_valid[patch] = 1;
-}
-
-/* fill_holes with the count Surface::expand returns */
-__global__ void
-fill_holes_count_kernel (int npx, int npy,
-    uint8_t const* __restrict__ node_valid, uint8_t* __restrict__ patch_valid,
-    unsigned long long* __restrict__ counter)
+    uint8_t* __restrict__ patch_valid, unsigned long long* __restrict__ counter)
 {
     int const patch = blockIdx.x * blockDim.x + threadIdx.x;
     if (patch >= npx * npy || patch_valid[patch])
@@ -215,7 +198,8 @@ fill_holes_count_kernel (int npx, int npy,
         && node_valid[n0 + npx + 2])
     {
         patch_valid[patch] = 1;
-        atomicAdd(counter, 1ull);
+        if (counter != nullptr)
+            atomicAdd(counter, 1ull);
     }
 }
 
@@ -492,7 +476,7 @@ topo_fill_from_depth (smvsb_ctx* c)
         count_launches(c, 1);
     }
     fill_holes_kernel<<<(np + 255) / 256, 256, 0, c->stream>>>(c->npx, c->npy,
-        c->node_valid.p, c->patch_valid.p);
+        c->node_valid.p, c->patch_valid.p, nullptr);
     CUDA_CHECK(cudaGetLastError());
     count_launches(c, 1);
     launch_remove_nodes(c);
@@ -575,7 +559,8 @@ topo_subdivide_finish (smvsb_ctx* c)
         cudaMemcpyDeviceToDevice, c->stream));
     CUDA_CHECK(cudaMemsetAsync(c->patch_valid.p, 0, np, c->stream));
     fill_holes_kernel<<<static_cast<unsigned>((np + 255) / 256), 256, 0,
-        c->stream>>>(c->npx, c->npy, c->node_valid.p, c->patch_valid.p);
+        c->stream>>>(c->npx, c->npy, c->node_valid.p, c->patch_valid.p,
+        nullptr);
     CUDA_CHECK(cudaGetLastError());
     count_launches(c, 1);
     launch_remove_nodes(c);
@@ -614,7 +599,7 @@ topo_expand (smvsb_ctx* c)
             c->node_valid_tmp.p, c->nodes_tmp.p, c->nodes.p,
             c->node_valid.p);
     }
-    fill_holes_count_kernel<<<(np + 255) / 256, 256, 0, c->stream>>>(c->npx,
+    fill_holes_kernel<<<(np + 255) / 256, 256, 0, c->stream>>>(c->npx,
         c->npy, c->node_valid.p, c->patch_valid.p, c->counters.p);
     CUDA_CHECK(cudaGetLastError());
     count_launches(c, 5);

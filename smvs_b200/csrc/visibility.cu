@@ -145,12 +145,62 @@ warp_anisotropy (double const* cf, double const* __restrict__ Mt, int px0,
     return worst;
 }
 
-/* second pass, :502-583: one thread per (patch, neighbour) */
+/* The per-pixel test of the second pass (:520-540): the pixel's projection
+ * into neighbour sub lies inside its 3 % border and is not behind its depth
+ * cache. */
+struct NeighbourTest
+{
+    unsigned int const* z;
+    int sw, sh;
+    double cut, hi_x, hi_y;
+
+    __device__ __forceinline__
+    NeighbourTest (VisArgs const& a, int sub)
+        : z(a.zbuf + a.zoff[sub]), sw(a.s.sub_dims[2 * sub]),
+          sh(a.s.sub_dims[2 * sub + 1])
+    {
+        cut = (xd(0.03) * xd(static_cast<double>(max(sw, sh)))).v;
+        hi_x = (xd(static_cast<double>(sw)) - xd(cut)).v;
+        hi_y = (xd(static_cast<double>(sh)) - xd(cut)).v;
+    }
+
+    __device__ __forceinline__ bool
+    passes (Warp const& c) const
+    {
+        if (!(c.projx >= cut && c.projx < hi_x
+            && c.projy >= cut && c.projy < hi_y))
+            return false;
+        int const cx = static_cast<int>(c.projx);
+        int const cy = static_cast<int>(c.projy);
+        double const near = (xd(c.depth) * xd(0.95)).v;
+        bool visible = true;
+        for (int dy = -1; dy < 2; ++dy)
+            for (int dx = -1; dx < 2; ++dx)
+            {
+                int const zx = cx + dx, zy = cy + dy;
+                if (zx < 0 || zy < 0 || zx > sw || zy > sh)
+                    continue;
+                float const zc = key_float(z[static_cast<size_t>(zy)
+                    * (sw + 1) + zx]);
+                if (near > static_cast<double>(zc))
+                    visible = false;
+            }
+        return visible;
+    }
+};
+
+/* second pass, :502-583: L lanes per (patch, neighbour). L = 32 serves the
+ * coarse scales (patch size 8 .. 64 pixels, a few thousand patches), where
+ * one thread per pair would leave the GPU to a handful of threads that each
+ * walk up to 4096 pixels. All three tests are order-free (every pixel
+ * passes / largest ratio), so the lanes take the pixels in turn. */
+template <int L>
 __global__ void __launch_bounds__(128)
 vis_patch_kernel (VisArgs const a)
 {
     SurfaceDev const& sf = a.s;
-    int const t = blockIdx.x * blockDim.x + threadIdx.x;
+    int const t = (blockIdx.x * blockDim.x + threadIdx.x) / L;
+    int const lane = threadIdx.x % L;
     if (t >= sf.npx * sf.npy * sf.n_sub)
         return;
     int const patch = t / sf.n_sub, sub = t % sf.n_sub;
@@ -162,111 +212,25 @@ vis_patch_kernel (VisArgs const a)
     load_patch_theta(sf.nodes, sf.npx, idx, idy, theta);
     patch_coefficients(theta, cf);
     double const* Mt = sf.Mt + sub * 12;
-    int const sw = sf.sub_dims[2 * sub], sh = sf.sub_dims[2 * sub + 1];
     int const px0 = sf.start_x + idx * ps, py0 = sf.start_y + idy * ps;
-    unsigned int const* z = a.zbuf + a.zoff[sub];
-
-    /* inside the neighbour (3 % border) and not behind its cache */
-    double const cut = (xd(0.03) * xd(static_cast<double>(max(sw, sh)))).v;
-    double const hi_x = (xd(static_cast<double>(sw)) - xd(cut)).v;
-    double const hi_y = (xd(static_cast<double>(sh)) - xd(cut)).v;
-    for (int pid = 0; pid < ps * ps; ++pid)
-    {
-        int const i = pid % ps, j = pid / ps;
-        PatchSample const smp = patch_sample<false>(cf, i, j, ps);
-        Warp const c = warp_pixel<false>(Mt, px0 + i + 0.5, py0 + j + 0.5,
-            smp.w, 0.0, 0.0);
-        if (!(c.projx >= cut && c.projx < hi_x
-            && c.projy >= cut && c.projy < hi_y))
-            return;
-        int const cx = static_cast<int>(c.projx);
-        int const cy = static_cast<int>(c.projy);
-        double const near = (xd(c.depth) * xd(0.95)).v;
-        for (int dy = -1; dy < 2; ++dy)
-            for (int dx = -1; dx < 2; ++dx)
-            {
-                int const zx = cx + dx, zy = cy + dy;
-                if (zx < 0 || zy < 0 || zx > sw || zy > sh)
-                    continue;
-                float const zc = key_float(z[static_cast<size_t>(zy)
-                    * (sw + 1) + zx]);
-                if (near > static_cast<double>(zc))
-                    return;
-            }
-    }
-
-    double const worst = warp_anisotropy(cf, Mt, px0, py0, ps);
-    if (worst > 8.0)
-        return;
-    atomicOr(a.vis_mask + patch, 1u << sub);
-}
-
-
-/* The same decisions with one WARP per (patch, neighbour): at the coarse
- * scales (patch size 8 .. 64 pixels, a few thousand patches) one thread per
- * pair leaves the GPU to a handful of threads that each walk up to 4096
- * pixels. All three tests are order-free (every pixel passes / largest
- * ratio), so the lanes take the pixels in turn. */
-__global__ void __launch_bounds__(128)
-vis_patch_warp_kernel (VisArgs const a)
-{
-    SurfaceDev const& sf = a.s;
-    int const t = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-    int const lane = threadIdx.x & 31;
-    if (t >= sf.npx * sf.npy * sf.n_sub)
-        return;
-    int const patch = t / sf.n_sub, sub = t % sf.n_sub;
-    if (!sf.patch_valid[patch])
-        return;
-    int const idx = patch % sf.npx, idy = patch / sf.npx;
-    int const ps = sf.ps;
-    double theta[16], cf[16];
-    load_patch_theta(sf.nodes, sf.npx, idx, idy, theta);
-    patch_coefficients(theta, cf);
-    double const* Mt = sf.Mt + sub * 12;
-    int const sw = sf.sub_dims[2 * sub], sh = sf.sub_dims[2 * sub + 1];
-    int const px0 = sf.start_x + idx * ps, py0 = sf.start_y + idy * ps;
-    unsigned int const* z = a.zbuf + a.zoff[sub];
-    double const cut = (xd(0.03) * xd(static_cast<double>(max(sw, sh)))).v;
-    double const hi_x = (xd(static_cast<double>(sw)) - xd(cut)).v;
-    double const hi_y = (xd(static_cast<double>(sh)) - xd(cut)).v;
+    NeighbourTest const test(a, sub);
     bool fail = false;
-    for (int pid = lane; pid < ps * ps && !fail; pid += 32)
+    for (int pid = lane; pid < ps * ps && !fail; pid += L)
     {
         int const i = pid % ps, j = pid / ps;
         PatchSample const smp = patch_sample<false>(cf, i, j, ps);
-        Warp const c = warp_pixel<false>(Mt, px0 + i + 0.5, py0 + j + 0.5,
-            smp.w, 0.0, 0.0);
-        if (!(c.projx >= cut && c.projx < hi_x
-            && c.projy >= cut && c.projy < hi_y))
-        {
-            fail = true;
-            break;
-        }
-        int const cx = static_cast<int>(c.projx);
-        int const cy = static_cast<int>(c.projy);
-        double const near = (xd(c.depth) * xd(0.95)).v;
-        for (int dy = -1; dy < 2; ++dy)
-            for (int dx = -1; dx < 2; ++dx)
-            {
-                int const zx = cx + dx, zy = cy + dy;
-                if (zx < 0 || zy < 0 || zx > sw || zy > sh)
-                    continue;
-                float const zc = key_float(z[static_cast<size_t>(zy)
-                    * (sw + 1) + zx]);
-                if (near > static_cast<double>(zc))
-                    fail = true;
-            }
+        fail = !test.passes(warp_pixel<false>(Mt, px0 + i + 0.5,
+            py0 + j + 0.5, smp.w, 0.0, 0.0));
     }
-    if (__any_sync(0xffffffffu, fail))
+    if (L == 1 ? fail : __any_sync(0xffffffffu, fail))
         return;
     double worst = 0.0;
-    for (int pid = lane; pid < ps * ps; pid += 32)
+    for (int pid = lane; pid < ps * ps; pid += L)
     {
         double const ratio = warp_anisotropy_at(cf, Mt, px0, py0, ps, pid);
-        worst = (worst < ratio) ? ratio : worst;
+        worst = (worst < ratio) ? ratio : worst;        /* std::max */
     }
-    for (int off = 16; off > 0; off >>= 1)
+    for (int off = L / 2; off > 0; off >>= 1)
     {
         double const other = __shfl_xor_sync(0xffffffffu, worst, off);
         worst = (worst < other) ? other : worst;
@@ -458,38 +422,14 @@ vis_patch_ncc_kernel (VisArgs const a)
     for (int sub = 0; sub < sf.n_sub; ++sub)
     {
         double const* Mt = sf.Mt + sub * 12;
-        int const sw = sf.sub_dims[2 * sub], sh = sf.sub_dims[2 * sub + 1];
-        unsigned int const* z = a.zbuf + a.zoff[sub];
-        double const cut = (xd(0.03) * xd(static_cast<double>(max(sw, sh)))).v;
-        double const hi_x = (xd(static_cast<double>(sw)) - xd(cut)).v;
-        double const hi_y = (xd(static_cast<double>(sh)) - xd(cut)).v;
+        NeighbourTest const test(a, sub);
         int const n_list = extended ? n_long : ps * ps;
         bool success = true;
         for (int i = 0; i < n_list && success; ++i)
         {
             ListEntry const e = list_entry(rim, i, ps, cf, theta, px0, py0);
-            Warp const c = warp_pixel<false>(Mt, (xd(e.x) + xd(0.5)).v,
-                (xd(e.y) + xd(0.5)).v, e.depth, 0.0, 0.0);
-            if (!(c.projx >= cut && c.projx < hi_x
-                && c.projy >= cut && c.projy < hi_y))
-            {
-                success = false;
-                break;
-            }
-            int const cx = static_cast<int>(c.projx);
-            int const cy = static_cast<int>(c.projy);
-            double const near = (xd(c.depth) * xd(0.95)).v;
-            for (int dy = -1; dy < 2; ++dy)
-                for (int dx = -1; dx < 2; ++dx)
-                {
-                    int const zx = cx + dx, zy = cy + dy;
-                    if (zx < 0 || zy < 0 || zx > sw || zy > sh)
-                        continue;
-                    float const zc = key_float(z[static_cast<size_t>(zy)
-                        * (sw + 1) + zx]);
-                    if (near > static_cast<double>(zc))
-                        success = false;
-                }
+            success = test.passes(warp_pixel<false>(Mt, (xd(e.x)
+                + xd(0.5)).v, (xd(e.y) + xd(0.5)).v, e.depth, 0.0, 0.0));
         }
         if (!success)
             continue;
@@ -549,7 +489,8 @@ remove_nodes_kernel (int npx, int npy, uint8_t const* __restrict__ patch_valid,
         node_valid[node] = 0;
 }
 
-/* exclusive prefix sum of counts[0..n) into off[0..n], one block */
+/* exclusive prefix sum of counts[0..n) into off[0..n), and the total into
+ * off[n]; one block */
 __global__ void __launch_bounds__(1024)
 scan_kernel (uint32_t const* __restrict__ counts, uint32_t* __restrict__ off,
     int n)
@@ -735,51 +676,18 @@ mse_term (SurfaceDev const& sf, double const* cf, int px0, int py0, int ps,
 }
 
 /* high photometric error at the rim of the surface, :402-428 with
- * mse_for_patch :747-793 */
+ * mse_for_patch :747-793; L lanes per patch (32 at the coarse scales, see
+ * vis_patch_kernel). mse_for_patch is a sequential sum (pixels outer,
+ * neighbours inner); the lanes evaluate L terms at a time and the terms are
+ * then added one after the other in that order (every lane keeps the same
+ * running sum), so the sum is bitwise the one-thread sum. */
+template <int L>
 __global__ void __launch_bounds__(128)
 cut_border_kernel (CutArgs const a)
 {
     SurfaceDev const& sf = a.s;
-    int const patch = blockIdx.x * blockDim.x + threadIdx.x;
-    if (patch >= sf.npx * sf.npy || !a.patch_valid[patch])
-        return;
-    int const idx = patch % sf.npx, idy = patch / sf.npx;
-    if (!patch_at_rim(sf, idx, idy))
-        return;
-
-    double theta[16], cf[16];
-    load_patch_theta(sf.nodes, sf.npx, idx, idy, theta);
-    patch_coefficients(theta, cf);
-    int const ps = sf.ps;
-    int const px0 = sf.start_x + idx * ps, py0 = sf.start_y + idy * ps;
-    uint32_t const v0 = sf.vis_off[patch];
-    int const n = static_cast<int>(sf.vis_off[patch + 1] - v0);
-    xd error(0.0), counter(0.0);
-    for (int pid = 0; pid < ps * ps; ++pid)
-        for (int k = 0; k < n; ++k)
-        {
-            error += mse_term(sf, cf, px0, py0, ps, pid, sf.vis_ids[v0 + k]);
-            counter += xd(1.0);
-        }
-    double const mse = (counter.v == 0.0) ? 1.0 : (error / counter).v;
-    if (mse > 0.05)
-    {
-        a.patch_valid[patch] = 0;
-        atomicAdd(a.counters, 1ull);
-    }
-}
-
-/* The same with one WARP per patch, for the coarse scales (see
- * vis_patch_warp_kernel). mse_for_patch is a sequential sum (pixels outer,
- * neighbours inner); the lanes evaluate 32 terms at a time and the terms are
- * then added one after the other in that order (every lane keeps the same
- * running sum), so the sum is bitwise the one-thread sum. */
-__global__ void __launch_bounds__(128)
-cut_border_warp_kernel (CutArgs const a)
-{
-    SurfaceDev const& sf = a.s;
-    int const patch = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-    int const lane = threadIdx.x & 31;
+    int const patch = (blockIdx.x * blockDim.x + threadIdx.x) / L;
+    int const lane = threadIdx.x % L;
     if (patch >= sf.npx * sf.npy || !a.patch_valid[patch])
         return;
     int const idx = patch % sf.npx, idy = patch / sf.npx;
@@ -794,16 +702,25 @@ cut_border_warp_kernel (CutArgs const a)
     int const n = static_cast<int>(sf.vis_off[patch + 1] - v0);
     int const total = ps * ps * n;
     xd error(0.0);
-    for (int base = 0; base < total; base += 32)
+    if constexpr (L == 1)
     {
-        int const t = base + lane;
-        double term = 0.0;
-        if (t < total)
-            term = mse_term(sf, cf, px0, py0, ps, t / n,
-                sf.vis_ids[v0 + t % n]).v;
-        int const m = min(32, total - base);
-        for (int l = 0; l < m; ++l)
-            error += xd(__shfl_sync(0xffffffffu, term, l));
+        for (int pid = 0; pid < ps * ps; ++pid)
+            for (int k = 0; k < n; ++k)
+                error += mse_term(sf, cf, px0, py0, ps, pid,
+                    sf.vis_ids[v0 + k]);
+    }
+    else
+    {
+        for (int base = 0; base < total; base += L)
+        {
+            int const t = base + lane;
+            double term = 0.0;
+            if (t < total)
+                term = mse_term(sf, cf, px0, py0, ps, t / n,
+                    sf.vis_ids[v0 + t % n]).v;
+            for (int l = 0; l < min(L, total - base); ++l)
+                error += xd(__shfl_sync(0xffffffffu, term, l));
+        }
     }
     double const counter = static_cast<double>(total);
     double const mse = (total == 0) ? 1.0 : (error / xd(counter)).v;
@@ -823,6 +740,15 @@ launch_remove_nodes (smvsb_ctx* c)
 {
     remove_nodes_kernel<<<(c->n_nodes + 255) / 256, 256, 0, c->stream>>>(
         c->npx, c->npy, c->patch_valid.p, c->node_valid.p);
+    CUDA_CHECK(cudaGetLastError());
+    smvsb::count_launches(c, 1);
+}
+
+void
+launch_exclusive_scan (smvsb_ctx* c, uint32_t const* counts, uint32_t* off,
+    int n)
+{
+    scan_kernel<<<1, 1024, 0, c->stream>>>(counts, off, n);
     CUDA_CHECK(cudaGetLastError());
     smvsb::count_launches(c, 1);
 }
@@ -953,19 +879,19 @@ run_visibility_device (smvsb_ctx* c, bool use_sgm)
         0, c->stream>>>(a);
     int const nt = np * c->n_sub;
     if (use_sgm && c->ps >= 8)
-        vis_patch_warp_kernel<<<(nt + 3) / 4, 128, 0, c->stream>>>(a);
+        vis_patch_kernel<32><<<(nt + 3) / 4, 128, 0, c->stream>>>(a);
     else if (use_sgm)
-        vis_patch_kernel<<<(nt + 127) / 128, 128, 0, c->stream>>>(a);
+        vis_patch_kernel<1><<<(nt + 127) / 128, 128, 0, c->stream>>>(a);
     else
         vis_patch_ncc_kernel<<<(np + 127) / 128, 128, 0, c->stream>>>(a);
     vis_finalize_kernel<<<(np + 255) / 256, 256, 0, c->stream>>>(a,
         c->patch_valid.p, c->vis_counts.p);
-    remove_nodes_kernel<<<(c->n_nodes + 255) / 256, 256, 0, c->stream>>>(
-        c->npx, c->npy, c->patch_valid.p, c->node_valid.p);
-    scan_kernel<<<1, 1024, 0, c->stream>>>(c->vis_counts.p, c->vis_off.p, np);
+    CUDA_CHECK(cudaGetLastError());
+    launch_remove_nodes(c);
+    launch_exclusive_scan(c, c->vis_counts.p, c->vis_off.p, np);
     vis_lists_kernel<<<(np + 255) / 256, 256, 0, c->stream>>>(np,
         c->vis_mask.p, c->vis_counts.p, c->vis_off.p, c->vis_ids.p);
-    smvsb::count_launches(c, 7);
+    smvsb::count_launches(c, 5);
     CUDA_CHECK(cudaGetLastError());
 
     unsigned long long removed = 0;
@@ -990,13 +916,12 @@ run_cut_boundaries (smvsb_ctx* c, float const* inv_calib)
     int const np = c->n_patches;
     cut_depth_kernel<<<(np + 255) / 256, 256, 0, c->stream>>>(a);
     if (c->ps >= 8)
-        cut_border_warp_kernel<<<(np + 3) / 4, 128, 0, c->stream>>>(a);
+        cut_border_kernel<32><<<(np + 3) / 4, 128, 0, c->stream>>>(a);
     else
-        cut_border_kernel<<<(np + 127) / 128, 128, 0, c->stream>>>(a);
-    remove_nodes_kernel<<<(c->n_nodes + 255) / 256, 256, 0, c->stream>>>(
-        c->npx, c->npy, c->patch_valid.p, c->node_valid.p);
-    smvsb::count_launches(c, 3);
+        cut_border_kernel<1><<<(np + 127) / 128, 128, 0, c->stream>>>(a);
     CUDA_CHECK(cudaGetLastError());
+    launch_remove_nodes(c);
+    smvsb::count_launches(c, 2);
     unsigned long long deleted = 0;
     CUDA_CHECK(cudaMemcpyAsync(&deleted, c->counters.p, sizeof(deleted),
         cudaMemcpyDeviceToHost, c->stream));
