@@ -142,6 +142,7 @@ int smvsb_debug_get_view (smvsb_ctx* ctx, int view, float* grad, float* hess);
  * The Surface and the per-patch visibility lists (DepthOptimizer::subsurfaces).
  *   scale, npx, npy, start_x, start_y   grid of lib/surface.cc:28-37: patch
  *       (idx, idy) has id idy*npx+idx, covers pixels start + id*2^scale;
+ *       scale 0..8 (patch size 1..256), larger is SMVSB_ERR_INVALID;
  *       node (idx, idy) has id idy*(npx+1)+idx (lib/surface.h:199-203)
  *   nodes        (npx+1)*(npy+1)*4   f, dx, dy, dxy per node (lib/bicubic_patch.h:29-36)
  *   node_valid   (npx+1)*(npy+1)     0 where Surface::nodes[i] == nullptr
@@ -319,6 +320,7 @@ int smvsb_get_surface_state (smvsb_ctx* ctx, uint8_t* node_valid,
  * initialize_node_from_depth :665-760, fill_holes :628-649,
  * remove_nodes_without_patch :762-867): the context's surface becomes the
  * surface of `scale` initialised from init_depth (w*h floats, 0 = no depth).
+ * scale 0..8, larger is SMVSB_ERR_INVALID.
  */
 int smvsb_surface_create (smvsb_ctx* ctx, int scale, const float* init_depth);
 /* Surface::subdivide_patches (lib/surface.cc:983-1107): the surface moves to
@@ -375,7 +377,9 @@ typedef struct smvsb_optimize_stats
  * convergence test, subdivision and hole filling between scales, lighting fit
  * below scale 4 with use_shading. The view stays on the device from the byte
  * images to the depth and normal maps; nothing but scalars comes back in
- * between.
+ * between. The ladder starts at max(ceil(log2(w*h / 1.7e6) / 2) + 4, 4)
+ * (:38-39), one scale coarser with no_sgm (:50); a start above scale 8
+ * (above 435 MP, 108.8 MP with no_sgm) is SMVSB_ERR_INVALID.
  *   inv_calib9    main camera's fill_inverse_calibration(w, h)
  *   shading, shading_grad   StereoView::get_shading_image / _gradients
  *                 (w*h, w*h*2) or NULL without use_shading

@@ -324,14 +324,21 @@ construct (smvsb_ctx* c, double const* light16, double reg, double light_reg)
     c->have_system = true;
 }
 
+/* Surfaces exist at scales 0..SMVSB_MAX_SCALE (patch sizes 1..256). */
+void
+require_surface_scale (int scale)
+{
+    require(scale >= 0 && scale <= SMVSB_MAX_SCALE, SMVSB_ERR_INVALID,
+        "surface scale out of range (0..8)");
+}
+
 /* Grid geometry of a Surface at `scale` (lib/surface.cc:28-37) and the tables
  * that depend on it. */
 void
 configure_grid (smvsb_ctx* c, int scale, int npx, int npy, int start_x,
     int start_y)
 {
-    require(scale >= 0 && scale <= 6, SMVSB_ERR_INVALID,
-        "scale out of range (0..6)");
+    require_surface_scale(scale);
     require(npx > 0 && npy > 0, SMVSB_ERR_INVALID, "empty patch grid");
     int const ps = 1 << scale;
     int const sampling = sampling_for_scale(scale);
@@ -339,7 +346,8 @@ configure_grid (smvsb_ctx* c, int scale, int npx, int npy, int start_x,
         "patch size below sampling");
     int const npos = ps / sampling;
     require(npos == 1 || npos == 2 || npos == 4 || npos == 8
-        || npos == 16, SMVSB_ERR_INVALID, "unsupported samples per patch");
+        || npos == 16 || npos == 32 || npos == 64, SMVSB_ERR_INVALID,
+        "unsupported samples per patch");
     require(start_x >= 0 && start_y >= 0
         && start_x + npx * ps <= c->w && start_y + npy * ps <= c->h,
         SMVSB_ERR_INVALID, "patch grid exceeds the main image");
@@ -384,6 +392,7 @@ clear_visibility (smvsb_ctx* c)
 void
 surface_create_device (smvsb_ctx* c, int scale, float const* init_dev)
 {
+    require_surface_scale(scale);
     int const ps = 1 << scale;
     int const npx = (c->w - 2) / ps - 1, npy = (c->h - 2) / ps - 1;
     require(npx > 0 && npy > 0, SMVSB_ERR_INVALID,
@@ -833,8 +842,7 @@ smvsb_set_surface (smvsb_ctx* ctx, int scale, int npx, int npy, int start_x,
     return guarded(ctx, [&]() {
         require(ctx->have_views, SMVSB_ERR_STATE,
             "smvsb_set_views must precede smvsb_set_surface");
-        require(scale >= 0 && scale <= 6, SMVSB_ERR_INVALID,
-            "scale out of range (0..6)");
+        require_surface_scale(scale);
         require(npx > 0 && npy > 0, SMVSB_ERR_INVALID, "empty patch grid");
         require(nodes && node_valid && patch_valid, SMVSB_ERR_INVALID,
             "surface arrays missing");
@@ -1346,8 +1354,8 @@ optimize_resident (smvsb_ctx* ctx, int w, int h, double flen_px,
             "no_sgm: the initial depth must have the size of the main view");
         int const init_scale = static_cast<int>(std::max(std::ceil(std::log2(
             w * h / 1.7e6) / 2) + 4, 4.0)) + (no_sgm ? 1 : 0);   /* :37-38, :51 */
-        require(init_scale <= 6, SMVSB_ERR_INVALID,
-            "image too large: initial scale above 6");
+        require(init_scale <= SMVSB_MAX_SCALE, SMVSB_ERR_INVALID,
+            "image too large: initial scale above 8");
         if (no_sgm)
         {
             /* the sparse depth of the bundle's features (lib/surface.cc:91-128)

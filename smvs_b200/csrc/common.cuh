@@ -16,6 +16,7 @@
 #include "../../include/smvs_b200.h"
 
 #define SMVSB_MAX_SUBS 32          /* neighbours per reference view */
+#define SMVSB_MAX_SCALE 8          /* coarsest surface scale (patch size 256) */
 #define SMVSB_NB_STRIDE 8          /* floats per packed neighbour texel */
 #define SMVSB_NUM_EVENTS 6
 

@@ -45,6 +45,57 @@ namespace smvsb {
 
 namespace {
 
+/* The tail of initialize_node_from_depth (lib/surface.cc:716-759) once the
+ * window is reduced to its quadrant counts and minima and the median of its
+ * n >= 2 depths: f = the median, the derivatives from the minima (a quadrant
+ * without depth counts as 0). */
+__device__ __forceinline__ void
+write_node (int node, int const* cnt, float const* qmin, float med,
+    uint8_t* __restrict__ node_valid, double* __restrict__ nodes)
+{
+    int num_non_zeros = 4;
+    double avg[4];
+    for (int q = 0; q < 4; ++q)
+    {
+        if (cnt[q] == 0)
+        {
+            avg[q] = 0.0;
+            num_non_zeros -= 1;
+        }
+        else
+            avg[q] = static_cast<double>(qmin[q]);
+    }
+    double const f = static_cast<double>(med);
+    double dx = 0.0, dy = 0.0, dxy = 0.0;
+    if (num_non_zeros == 4)
+    {
+        dx = __ddiv_rn(__dadd_rn(__dadd_rn(avg[1], avg[3]),
+            -__dadd_rn(avg[0], avg[2])), 2.0);
+        dy = __ddiv_rn(__dadd_rn(__dadd_rn(avg[2], avg[3]),
+            -__dadd_rn(avg[0], avg[1])), 2.0);
+        dxy = __dadd_rn(__dadd_rn(avg[3], -avg[2]),
+            -__dadd_rn(avg[1], -avg[0]));
+    }
+    else
+    {
+        if ((avg[1] == 0 || avg[0] == 0) && avg[3] != 0 && avg[2] != 0)
+            dx = __dadd_rn(avg[3], -avg[2]);
+        else if ((avg[2] == 0 || avg[3] == 0) && avg[1] != 0
+            && avg[0] != 0)
+            dx = __dadd_rn(avg[1], -avg[0]);
+        if ((avg[0] == 0 || avg[2] == 0) && avg[3] != 0 && avg[1] != 0)
+            dy = __dadd_rn(avg[3], -avg[1]);
+        else if ((avg[1] == 0 || avg[2] == 0) && avg[0] != 0
+            && avg[2] != 0)
+            dy = __dadd_rn(avg[2], -avg[0]);
+    }
+    nodes[static_cast<size_t>(node) * 4 + 0] = f;
+    nodes[static_cast<size_t>(node) * 4 + 1] = dx;
+    nodes[static_cast<size_t>(node) * 4 + 2] = dy;
+    nodes[static_cast<size_t>(node) * 4 + 3] = dxy;
+    node_valid[node] = 1;
+}
+
 /* One warp per node. Window values (floats) are gathered into shared memory,
  * per-quadrant minima by warp reduction, the median by ranking: the element
  * std::nth_element(all.begin(), all.begin() + n / 2, all.end()) leaves at
@@ -112,19 +163,7 @@ init_nodes_kernel (int npx, int npy, int ps, int sx, int sy, int w, int h,
     }
     __syncwarp();
 
-    int num_non_zeros = 4;
-    double avg[4];
-    for (int q = 0; q < 4; ++q)
-    {
-        if (cnt[q] == 0)
-        {
-            avg[q] = 0.0;
-            num_non_zeros -= 1;
-        }
-        else
-            avg[q] = static_cast<double>(qmin[q]);
-    }
-    if (num_non_zeros == 0 || n < 2)
+    if (n < 2)          /* n >= 2: some quadrant has depth */
         return;
 
     /* median: element with rank n / 2 */
@@ -150,36 +189,122 @@ init_nodes_kernel (int npx, int npy, int ps, int sx, int sy, int w, int h,
     med = __shfl_sync(0xffffffffu, med, __ffs(who) - 1);
 
     if (lane == 0)
+        write_node(node, cnt, qmin, med, node_valid, nodes);
+}
+
+/* The same for windows that do not fit in shared memory (patch size 128 and
+ * 256, scales 7 and 8: 16 K and 64 K depths per node): one block per node
+ * re-reads the window from the depth image. One pass counts each quadrant's
+ * depths and takes its minimum; the median is then found by radix selection
+ * over the fp32 bits, eight bits per pass. The depths are positive, so their
+ * bits order like their values, and after four passes the selected bits are
+ * the value with exactly n / 2 depths below it in the sorted order -- the
+ * element std::nth_element leaves at n / 2. Counts, minima and histograms are
+ * order-free, so the result does not depend on the thread schedule. */
+constexpr int SELECT_THREADS = 256;
+
+__global__ void __launch_bounds__(SELECT_THREADS)
+init_nodes_select_kernel (int npx, int npy, int ps, int sx, int sy, int w,
+    int h, float const* __restrict__ depth, uint8_t* __restrict__ node_valid,
+    double* __restrict__ nodes)
+{
+    __shared__ unsigned s_hist[256];
+    __shared__ int s_cnt[4];
+    __shared__ unsigned s_min[4];
+    __shared__ unsigned s_prefix;
+    __shared__ int s_rank;
+    int const tid = threadIdx.x;
+    int const node = blockIdx.x;
+    int const ns = npx + 1;
+    if (node_valid[node])
+        return;
+    int const idx = node % ns, idy = node / ns;
+    int const x = idx * ps + sx, y = idy * ps + sy;
+    int const win = ps / 2, side = 2 * win;
+
+    /* depth bits of window entry e (row-major over [-win, win)^2), 0 where
+     * the window leaves the image or has no depth */
+    auto bits_at = [&](int e) -> unsigned {
+        int const gx = x + e % side - win, gy = y + e / side - win;
+        if (gx < 0 || gx >= w || gy < 0 || gy >= h)
+            return 0u;
+        float const v = depth[static_cast<size_t>(gy) * w + gx];
+        return (v > 0.0f) ? __float_as_uint(v) : 0u;
+    };
+
+    if (tid < 4)
     {
-        double const f = static_cast<double>(med);
-        double dx = 0.0, dy = 0.0, dxy = 0.0;
-        if (num_non_zeros == 4)
+        s_cnt[tid] = 0;
+        s_min[tid] = 0xffffffffu;
+    }
+    for (int i = tid; i < 256; i += SELECT_THREADS)
+        s_hist[i] = 0;
+    __syncthreads();
+    int cnt[4] = {0, 0, 0, 0};
+    unsigned mn[4] = {0xffffffffu, 0xffffffffu, 0xffffffffu, 0xffffffffu};
+    for (int e = tid; e < side * side; e += SELECT_THREADS)
+    {
+        unsigned const b = bits_at(e);
+        if (b == 0u)
+            continue;
+        /* quadrant: bit 0 = right half (i >= 0), bit 1 = lower half */
+        int const q = (e % side >= win ? 1 : 0) + (e / side >= win ? 2 : 0);
+        cnt[q] += 1;
+        mn[q] = min(mn[q], b);
+        atomicAdd(&s_hist[b >> 24], 1u);
+    }
+    for (int q = 0; q < 4; ++q)
+    {
+        if (cnt[q] == 0)
+            continue;
+        atomicAdd(&s_cnt[q], cnt[q]);
+        atomicMin(&s_min[q], mn[q]);
+    }
+    __syncthreads();
+    int const n = s_cnt[0] + s_cnt[1] + s_cnt[2] + s_cnt[3];
+    if (n < 2)
+        return;
+
+    unsigned prefix = 0u;
+    int rank = n / 2;               /* rank among the depths matching prefix */
+    for (int shift = 24; ; shift -= 8)
+    {
+        if (tid == 0)
         {
-            dx = __ddiv_rn(__dadd_rn(__dadd_rn(avg[1], avg[3]),
-                -__dadd_rn(avg[0], avg[2])), 2.0);
-            dy = __ddiv_rn(__dadd_rn(__dadd_rn(avg[2], avg[3]),
-                -__dadd_rn(avg[0], avg[1])), 2.0);
-            dxy = __dadd_rn(__dadd_rn(avg[3], -avg[2]),
-                -__dadd_rn(avg[1], -avg[0]));
+            int below = 0, b = 0;
+            while (below + static_cast<int>(s_hist[b]) <= rank)
+                below += static_cast<int>(s_hist[b++]);
+            s_prefix = prefix | (static_cast<unsigned>(b) << shift);
+            s_rank = rank - below;
         }
-        else
+        __syncthreads();
+        prefix = s_prefix;
+        rank = s_rank;
+        if (shift == 0)
+            break;
+        for (int i = tid; i < 256; i += SELECT_THREADS)
+            s_hist[i] = 0;
+        __syncthreads();
+        unsigned const high = 0xffffffffu << shift;
+        for (int e = tid; e < side * side; e += SELECT_THREADS)
         {
-            if ((avg[1] == 0 || avg[0] == 0) && avg[3] != 0 && avg[2] != 0)
-                dx = __dadd_rn(avg[3], -avg[2]);
-            else if ((avg[2] == 0 || avg[3] == 0) && avg[1] != 0
-                && avg[0] != 0)
-                dx = __dadd_rn(avg[1], -avg[0]);
-            if ((avg[0] == 0 || avg[2] == 0) && avg[3] != 0 && avg[1] != 0)
-                dy = __dadd_rn(avg[3], -avg[1]);
-            else if ((avg[1] == 0 || avg[2] == 0) && avg[0] != 0
-                && avg[2] != 0)
-                dy = __dadd_rn(avg[2], -avg[0]);
+            unsigned const b = bits_at(e);
+            if (b != 0u && (b & high) == prefix)
+                atomicAdd(&s_hist[(b >> (shift - 8)) & 255u], 1u);
         }
-        nodes[static_cast<size_t>(node) * 4 + 0] = f;
-        nodes[static_cast<size_t>(node) * 4 + 1] = dx;
-        nodes[static_cast<size_t>(node) * 4 + 2] = dy;
-        nodes[static_cast<size_t>(node) * 4 + 3] = dxy;
-        node_valid[node] = 1;
+        __syncthreads();
+    }
+
+    if (tid == 0)
+    {
+        int c[4];
+        float qmin[4];
+        for (int q = 0; q < 4; ++q)
+        {
+            c[q] = s_cnt[q];
+            qmin[q] = __uint_as_float(s_min[q]);
+        }
+        write_node(node, c, qmin, __uint_as_float(prefix), node_valid, nodes);
     }
 }
 
@@ -460,7 +585,15 @@ topo_fill_from_depth (smvsb_ctx* c)
 {
     int const nn = c->n_nodes, np = c->n_patches;
     int const win = c->ps / 2;
-    if (win >= 1)
+    if (win > 32)
+    {
+        init_nodes_select_kernel<<<nn, SELECT_THREADS, 0, c->stream>>>(
+            c->npx, c->npy, c->ps, c->start_x, c->start_y, c->w, c->h,
+            c->init_depth.p, c->node_valid.p, c->nodes.p);
+        CUDA_CHECK(cudaGetLastError());
+        count_launches(c, 1);
+    }
+    else if (win >= 1)
     {
         size_t const smem = static_cast<size_t>(INIT_WARPS) * 4 * win * win
             * sizeof(float);

@@ -43,8 +43,10 @@ eval_depth (double const* theta, double const* X0, double const* Y0)
  * G = threads per patch (a power of two <= UPD_THREADS, = min(ps^2, 64));
  * a block holds UPD_THREADS / G patches, so at scale 2 (16 pixels per patch)
  * four patches share a block instead of leaving 48 of 64 threads idle.
+ * PS_MAX = the largest patch size the cached basis_f row holds (64 up to
+ * scale 6, 256 at scales 7 and 8).
  */
-template <int G>
+template <int G, int PS_MAX = 64>
 __global__ void __launch_bounds__(UPD_THREADS)
 reproj_kernel (SurfaceDev const sf, double const* __restrict__ delta,
     double thresh, uint8_t* __restrict__ active_new,
@@ -52,7 +54,7 @@ reproj_kernel (SurfaceDev const sf, double const* __restrict__ delta,
 {
     constexpr int PPB = UPD_THREADS / G;
     __shared__ double s_theta[PPB][16], s_dtheta[PPB][16];
-    __shared__ double s_b0[64 * 4];
+    __shared__ double s_b0[PS_MAX * 4];
     __shared__ double s_sum[UPD_THREADS / 32];
     __shared__ int s_flag[UPD_THREADS / 32];
 
@@ -350,7 +352,10 @@ update_enqueue (smvsb_ctx* c, double thresh, bool full_opt)
     int const npix_patch = c->ps * c->ps;
     auto grid_for = [&](int g) { int const ppb = UPD_THREADS / g;
         return (c->n_patches + ppb - 1) / ppb; };
-    if (npix_patch >= 64)
+    if (c->ps > 64)
+        reproj_kernel<64, 256><<<grid_for(64), UPD_THREADS, 0, c->stream>>>(
+            sf, c->x.p, thresh, c->active_new.p, c->patch_shift.p);
+    else if (npix_patch >= 64)
         reproj_kernel<64><<<grid_for(64), UPD_THREADS, 0, c->stream>>>(sf,
             c->x.p, thresh, c->active_new.p, c->patch_shift.p);
     else if (npix_patch == 16)

@@ -22,7 +22,9 @@ namespace smvsb {
 
 namespace {
 
-constexpr int BLUR_MAX_KS = 64;
+/* blur radius ceil(2.884 * (0.12 * 2^scale + 0.2)): 45 at scale 7, 90 at
+ * scale 8, the coarsest scale a surface starts at */
+constexpr int BLUR_MAX_KS = 90;
 
 struct BlurKernel
 {

@@ -292,7 +292,9 @@ list_entry (short4 const* __restrict__ rim, int i, int ps,
     else
     {
         short4 const e = rim[i - ps * ps];
-        ox = e.x; oy = e.y; src = e.z;
+        ox = e.x; oy = e.y;
+        src = static_cast<int>((static_cast<unsigned>(static_cast<uint16_t>(
+            e.w)) << 16) | static_cast<uint16_t>(e.z));
     }
     ListEntry out;
     out.x = static_cast<double>(px0 + ox);
@@ -383,17 +385,135 @@ ncc_for_patch_dev (VisArgs const& a, int sub, short4 const* rim, int n_list,
     return (s01 / (norm0 * norm1)).v;
 }
 
-/* second pass in the use_sgm = false mode: one thread per PATCH, neighbours
+/* ncc_for_patch_dev on the 32 lanes of a warp (patch sizes 128 and 256: a
+ * list of 16 K / 65 K entries). The lanes evaluate 32 entries at a time --
+ * the warp into the neighbour and the bilinear taps, which are the cost --
+ * and every lane then folds them into the running means, and in the second
+ * pass into the paired sums, one after the other in list order: the result is
+ * bitwise the sequential one. The reference returns -1 at the first entry
+ * whose projection leaves the image, whatever the entries before it gave, so
+ * "any entry leaves" is the same test. */
+__device__ double
+ncc_for_patch_warp (VisArgs const& a, int sub, short4 const* rim, int n_list,
+    int ps, double const* cf, double const* theta, int px0, int py0, int lane)
+{
+    SurfaceDev const& sf = a.s;
+    double const* Mt = sf.Mt + sub * 12;
+    int const sw = sf.sub_dims[2 * sub], sh = sf.sub_dims[2 * sub + 1];
+    float const* simg = a.color_subs[sub];
+    xd means0[3], means1[3], counter[3];
+    for (int c = 0; c < 3; ++c)
+        means0[c] = means1[c] = counter[c] = xd(0.0);
+    double const hi_x = static_cast<double>(sw - 2);
+    double const hi_y = static_cast<double>(sh - 2);
+    for (int base = 0; base < n_list; base += 32)
+    {
+        int const i = base + lane;
+        bool out = false;
+        double cm[3] = {0.0, 0.0, 0.0}, cs[3] = {0.0, 0.0, 0.0};
+        if (i < n_list)
+        {
+            ListEntry const e = list_entry(rim, i, ps, cf, theta, px0, py0);
+            Warp const c = warp_pixel<false>(Mt, (xd(e.x) + xd(0.5)).v,
+                (xd(e.y) + xd(0.5)).v, e.depth, 0.0, 0.0);
+            out = c.projx < 1 || c.projx > hi_x || c.projy < 1
+                || c.projy > hi_y;
+            if (!out)
+            {
+                size_t const mp = (static_cast<size_t>(static_cast<int>(e.y))
+                    * sf.w + static_cast<int>(e.x)) * 3;
+                for (int ch = 0; ch < 3; ++ch)
+                {
+                    cm[ch] = static_cast<double>(a.color_main[mp + ch]);
+                    cs[ch] = static_cast<double>(linear_at_rgb(simg, sw, sh,
+                        static_cast<float>(c.projx),
+                        static_cast<float>(c.projy), ch));
+                }
+            }
+        }
+        if (__any_sync(0xffffffffu, out))
+            return -1.0;
+        int const m = min(32, n_list - base);
+        for (int l = 0; l < m; ++l)
+            for (int ch = 0; ch < 3; ++ch)
+            {
+                xd const vm(__shfl_sync(0xffffffffu, cm[ch], l));
+                xd const vs(__shfl_sync(0xffffffffu, cs[ch], l));
+                counter[ch] += xd(1.0);
+                means0[ch] += (vm - means0[ch]) / counter[ch];
+                means1[ch] += (vs - means1[ch]) / counter[ch];
+            }
+    }
+    /* SSEVector::dot pairing as in ncc_for_patch_dev */
+    xd s00(0.0), s11(0.0), s01(0.0);
+    xd p00(0.0), p11(0.0), p01(0.0);
+    int k = 0;
+    for (int base = 0; base < n_list; base += 32)
+    {
+        int const i = base + lane;
+        double d0[3] = {0.0, 0.0, 0.0}, d1[3] = {0.0, 0.0, 0.0};
+        if (i < n_list)
+        {
+            ListEntry const e = list_entry(rim, i, ps, cf, theta, px0, py0);
+            Warp const c = warp_pixel<false>(Mt, (xd(e.x) + xd(0.5)).v,
+                (xd(e.y) + xd(0.5)).v, e.depth, 0.0, 0.0);
+            size_t const mp = (static_cast<size_t>(static_cast<int>(e.y))
+                * sf.w + static_cast<int>(e.x)) * 3;
+            for (int ch = 0; ch < 3; ++ch)
+            {
+                d0[ch] = (xd(static_cast<double>(a.color_main[mp + ch]))
+                    - means0[ch]).v;
+                d1[ch] = (xd(static_cast<double>(linear_at_rgb(simg, sw, sh,
+                    static_cast<float>(c.projx), static_cast<float>(c.projy),
+                    ch))) - means1[ch]).v;
+            }
+        }
+        int const m = min(32, n_list - base);
+        for (int l = 0; l < m; ++l)
+            for (int ch = 0; ch < 3; ++ch, ++k)
+            {
+                xd const v0(__shfl_sync(0xffffffffu, d0[ch], l));
+                xd const v1(__shfl_sync(0xffffffffu, d1[ch], l));
+                if ((k & 1) == 0)
+                {
+                    p00 = v0 * v0; p11 = v1 * v1; p01 = v0 * v1;
+                }
+                else
+                {
+                    s00 += p00 + v0 * v0;
+                    s11 += p11 + v1 * v1;
+                    s01 += p01 + v0 * v1;
+                }
+            }
+    }
+    if (k & 1)
+    {
+        s00 += p00; s11 += p11; s01 += p01;
+    }
+    xd const norm0 = xsqrt(s00), norm1 = xsqrt(s11);
+    if ((norm0 + norm1).v < (xd(0.001) * xd(static_cast<double>(n_list))).v)
+        return 1.0;
+    return (s01 / (norm0 * norm1)).v;
+}
+
+/* second pass in the use_sgm = false mode: L lanes per PATCH, neighbours
  * in order, because the reference's member vectors `pixels` / `depths` carry
  * state from one neighbour to the next (:508, :514, :551, :579): after
  * ncc_for_patch ran they hold the patch AND its rim, and the next
  * neighbour's border and depth tests run over that longer list until a
- * neighbour passes them (which resets the vectors to the patch's pixels). */
+ * neighbour passes them (which resets the vectors to the patch's pixels).
+ * L = 32 serves patch sizes 128 and 256 (scales 7 and 8), where one thread
+ * per patch would leave a few hundred threads to walk 16 K / 65 K pixels per
+ * neighbour: the lanes take the list entries in turn for the border / depth
+ * test (every entry passes) and the anisotropy (largest ratio), and
+ * ncc_for_patch_warp keeps the NCC's sequential sums. */
+template <int L>
 __global__ void __launch_bounds__(128)
 vis_patch_ncc_kernel (VisArgs const a)
 {
     SurfaceDev const& sf = a.s;
-    int const patch = blockIdx.x * blockDim.x + threadIdx.x;
+    int const patch = (blockIdx.x * blockDim.x + threadIdx.x) / L;
+    int const lane = threadIdx.x % L;
     if (patch >= sf.npx * sf.npy || !sf.patch_valid[patch])
         return;
     int const idx = patch % sf.npx, idy = patch / sf.npx;
@@ -425,24 +545,53 @@ vis_patch_ncc_kernel (VisArgs const a)
         NeighbourTest const test(a, sub);
         int const n_list = extended ? n_long : ps * ps;
         bool success = true;
-        for (int i = 0; i < n_list && success; ++i)
+        for (int base = 0; base < n_list && success; base += L)
         {
-            ListEntry const e = list_entry(rim, i, ps, cf, theta, px0, py0);
-            success = test.passes(warp_pixel<false>(Mt, (xd(e.x)
-                + xd(0.5)).v, (xd(e.y) + xd(0.5)).v, e.depth, 0.0, 0.0));
+            int const i = base + lane;
+            bool pass = true;
+            if (i < n_list)
+            {
+                ListEntry const e = list_entry(rim, i, ps, cf, theta, px0,
+                    py0);
+                pass = test.passes(warp_pixel<false>(Mt, (xd(e.x)
+                    + xd(0.5)).v, (xd(e.y) + xd(0.5)).v, e.depth, 0.0, 0.0));
+            }
+            success = (L == 1) ? pass : __all_sync(0xffffffffu, pass);
         }
         if (!success)
             continue;
         extended = false;           /* :551 refills the vectors */
-        if (warp_anisotropy(cf, Mt, px0, py0, ps) > 8.0)
+        double worst;
+        if constexpr (L == 1)
+            worst = warp_anisotropy(cf, Mt, px0, py0, ps);
+        else
+        {
+            worst = 0.0;
+            for (int pid = lane; pid < ps * ps; pid += L)
+            {
+                double const ratio = warp_anisotropy_at(cf, Mt, px0, py0, ps,
+                    pid);
+                worst = (worst < ratio) ? ratio : worst;    /* std::max */
+            }
+            for (int off = L / 2; off > 0; off >>= 1)
+            {
+                double const other = __shfl_xor_sync(0xffffffffu, worst, off);
+                worst = (worst < other) ? other : worst;
+            }
+        }
+        if (worst > 8.0)
             continue;
         extended = true;            /* ncc_for_patch leaves the rim in them */
-        if (ncc_for_patch_dev(a, sub, rim, n_long, ps, cf, theta, px0, py0)
-            < 0)
+        double const ncc = (L == 1)
+            ? ncc_for_patch_dev(a, sub, rim, n_long, ps, cf, theta, px0, py0)
+            : ncc_for_patch_warp(a, sub, rim, n_long, ps, cf, theta, px0, py0,
+                lane);
+        if (ncc < 0)
             continue;
         mask |= 1u << sub;
     }
-    a.vis_mask[patch] = mask;
+    if (lane == 0)
+        a.vis_mask[patch] = mask;
 }
 
 /* :585-600: patches no neighbour sees are deleted */
@@ -767,7 +916,9 @@ run_visibility (smvsb_ctx* c, float const* sgm_depth_host)
  * relative to the patch origin: entries beyond the patch's own ps * ps pixels
  * for each of the eight combinations of (corners fit, top rim fits, left rim
  * fits). Run exactly like the reference: the loop walks the list while it
- * grows. z = where the depth comes from (patch pixel index, or -1 - corner). */
+ * grows. Where the depth comes from (patch pixel index, or -1 - corner) is
+ * 32 bits, low half in z and high half in w: at patch size 256 a pixel index
+ * reaches 65 280. */
 static void
 build_rim_lists (int ps, std::vector<short4>* out, int* off)
 {
@@ -808,9 +959,13 @@ build_rim_lists (int ps, std::vector<short4>* out, int* off)
         }
         for (std::size_t i = static_cast<std::size_t>(ps) * ps;
             i < list.size(); ++i)
+        {
+            unsigned const src = static_cast<unsigned>(list[i].src);
             out->push_back(make_short4(static_cast<short>(list[i].x),
                 static_cast<short>(list[i].y),
-                static_cast<short>(list[i].src), 0));
+                static_cast<short>(static_cast<uint16_t>(src & 0xffffu)),
+                static_cast<short>(static_cast<uint16_t>(src >> 16))));
+        }
     }
     off[8] = static_cast<int>(out->size());
 }
@@ -882,8 +1037,10 @@ run_visibility_device (smvsb_ctx* c, bool use_sgm)
         vis_patch_kernel<32><<<(nt + 3) / 4, 128, 0, c->stream>>>(a);
     else if (use_sgm)
         vis_patch_kernel<1><<<(nt + 127) / 128, 128, 0, c->stream>>>(a);
+    else if (c->ps >= 128)
+        vis_patch_ncc_kernel<32><<<(np + 3) / 4, 128, 0, c->stream>>>(a);
     else
-        vis_patch_ncc_kernel<<<(np + 127) / 128, 128, 0, c->stream>>>(a);
+        vis_patch_ncc_kernel<1><<<(np + 127) / 128, 128, 0, c->stream>>>(a);
     vis_finalize_kernel<<<(np + 255) / 256, 256, 0, c->stream>>>(a,
         c->patch_valid.p, c->vis_counts.p);
     CUDA_CHECK(cudaGetLastError());
