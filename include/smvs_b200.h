@@ -465,7 +465,8 @@ int smvsb_fit_lighting (smvsb_ctx* ctx, double* params16_out,
  *   depth_out  w*h floats
  *   cost_out / sgm_out  optional w*h*num_steps uint16 dumps (NULL to skip)
  *   ms_out     optional double[3]: device ms of cost volume, aggregation, WTA
- * num_steps must be a multiple of 32 and <= 256.
+ * num_steps must be a multiple of 32 and <= 256. Runs within the default
+ * device budget (smvsb_sgm_ex with opts = NULL).
  */
 int smvsb_sgm (int device, int w, int h, const uint8_t* main_lum,
     int nw, int nh, const uint8_t* neigh_lum, const float* M, const float* t,
@@ -488,6 +489,8 @@ int smvsb_sgm (int device, int w, int h, const uint8_t* main_lum,
  *   depth_range_main / _neigh   {min, max} depth of the two runs (:50-61)
  *   merge_with   w*h floats or NULL
  *   ms_out       optional double[2]: device ms of the two run_sgm
+ * Runs within the default device budget (smvsb_sgm_reconstruct_ex with
+ * opts = NULL).
  */
 int smvsb_sgm_reconstruct (int device, int w, int h, const uint8_t* main_lum,
     int nw, int nh, const uint8_t* neigh_lum, const float* M_mn,
@@ -495,6 +498,61 @@ int smvsb_sgm_reconstruct (int device, int w, int h, const uint8_t* main_lum,
     const float* depth_range_main, const float* depth_range_neigh,
     int num_steps, uint16_t penalty1, uint16_t penalty2,
     const float* merge_with, float* depth_out, double* ms_out);
+
+/* Device memory of smvsb_sgm_ex and smvsb_sgm_reconstruct_ex. */
+typedef struct smvsb_sgm_options
+{
+    uint64_t device_bytes;       /* the device's SGM workspace holds at most
+                                    this much; 0 = the smaller of a quarter of
+                                    the card and its free memory (counting
+                                    what the workspace holds) less a margin
+                                    (1/32 of the card, >= 256 MiB) */
+    uint64_t reserved[3];        /* 0 */
+} smvsb_sgm_options;
+
+typedef struct smvsb_sgm_stats
+{
+    int32_t banded;              /* 1: a run took the banded path */
+    int32_t bands;               /* bands per run (the larger of a
+                                    reconstruct's two); 1 on the volume path */
+    uint64_t peak_device_bytes;  /* the workspace's largest size in the call */
+    uint64_t host_bytes;         /* partial sums staged in pinned host memory */
+    double ms_device;            /* CUDA events over the run_sgm calls */
+} smvsb_sgm_stats;
+
+/*
+ * smvsb_sgm and smvsb_sgm_reconstruct within a device-memory budget (the
+ * per-device workspace holds at most opts->device_bytes after the call).
+ * Each run_sgm keeps its whole cost and aggregation volumes on the device
+ * (about 10 bytes per voxel) when they fit the budget. Otherwise it runs in
+ * bands of image rows: cost per band (census halo recomputed), a top-to-bottom
+ * sweep of the downward and horizontal paths that keeps a uint16 partial sum
+ * per voxel (on the device, or in pinned host memory when the budget cannot
+ * hold it next to a useful band), and a bottom-to-top sweep of the upward
+ * paths that adds it and takes the winner. The depth is bit-identical
+ * whatever the path and budget. cost_out / sgm_out always take the volume
+ * path, whatever the budget. On the banded path the stages interleave:
+ * ms_out[0] of smvsb_sgm_ex is the whole run and ms_out[1..2] are 0.
+ *   opts    NULL = defaults
+ *   stats   may be NULL
+ * SMVSB_ERR_INVALID: a device_bytes budget too small for one band of 16 rows
+ * and the carried state (the message names the minimum); SMVSB_ERR_ALLOC:
+ * the default budget is that small, or the device has not that much memory.
+ */
+int smvsb_sgm_ex (int device, int w, int h, const uint8_t* main_lum,
+    int nw, int nh, const uint8_t* neigh_lum, const float* M, const float* t,
+    float min_depth, float max_depth, int num_steps, uint16_t penalty1,
+    uint16_t penalty2, float* depth_out, uint16_t* cost_out,
+    uint16_t* sgm_out, double* ms_out, const smvsb_sgm_options* opts,
+    smvsb_sgm_stats* stats);
+
+int smvsb_sgm_reconstruct_ex (int device, int w, int h,
+    const uint8_t* main_lum, int nw, int nh, const uint8_t* neigh_lum,
+    const float* M_mn, const float* t_mn, const float* M_nm,
+    const float* t_nm, const float* depth_range_main,
+    const float* depth_range_neigh, int num_steps, uint16_t penalty1,
+    uint16_t penalty2, const float* merge_with, float* depth_out,
+    double* ms_out, const smvsb_sgm_options* opts, smvsb_sgm_stats* stats);
 
 /* ---- after the per-view optimisation ------------------------------------ */
 

@@ -29,7 +29,7 @@ EXPORTS = [
     "smvsb_surface_fill_from_depth", "smvsb_surface_remove_isolated", "smvsb_surface_expand", "smvsb_surface_info",
     "smvsb_set_color_images",
     "smvsb_optimize", "smvsb_optimize_rgb_f32", "smvsb_view_set_scale_c", "smvsb_measure_fp64_peak", "smvsb_sgm_reconstruct", "smvsb_newton_loop_batch", "smvsb_device_launch_count",
-    "smvsb_cut_depth_maps_multi",
+    "smvsb_cut_depth_maps_multi", "smvsb_sgm_ex", "smvsb_sgm_reconstruct_ex",
 ]
 
 
@@ -426,9 +426,34 @@ def newton_loop_batch(ctxs, lights=None, regularization=0.01,
     return [_stats_dict(s) for s in st]
 
 
+class SgmOptions(C.Structure):
+    _fields_ = [("device_bytes", C.c_uint64), ("reserved", C.c_uint64 * 3)]
+
+
+class SgmStats(C.Structure):
+    _fields_ = [("banded", C.c_int32), ("bands", C.c_int32),
+                ("peak_device_bytes", C.c_uint64), ("host_bytes", C.c_uint64),
+                ("ms_device", C.c_double)]
+
+
+def _sgm_ex_args(device_bytes):
+    """The stats and the (options, stats) arguments of smvsb_sgm_ex /
+    smvsb_sgm_reconstruct_ex."""
+    st = SgmStats()
+    return st, (C.byref(SgmOptions(int(device_bytes))), C.byref(st))
+
+
+def _sgm_stats(st):
+    return {f: getattr(st, f) for f, _ in SgmStats._fields_}
+
+
 def sgm(main_lum, neigh_lum, M, t, min_depth, max_depth, num_steps=128,
-        penalty1=6, penalty2=96, device=0, volumes=False):
-    """SGMStereo::run_sgm for one luminance pair (smvsb_sgm)."""
+        penalty1=6, penalty2=96, device=0, volumes=False, *, device_bytes=0,
+        return_stats=False):
+    """SGMStereo::run_sgm for one luminance pair (smvsb_sgm).
+    device_bytes (a cap on the device's SGM workspace; 0 = the default budget)
+    or return_stats select smvsb_sgm_ex; with return_stats the result is
+    (dict, stats dict)."""
     main_lum, neigh_lum = _u8(main_lum), _u8(neigh_lum)
     h, w = main_lum.shape
     nh, nw = neigh_lum.shape
@@ -437,19 +462,27 @@ def sgm(main_lum, neigh_lum, M, t, min_depth, max_depth, num_steps=128,
     cost = np.empty((h, w, num_steps), dtype=np.uint16) if volumes else None
     S = np.empty((h, w, num_steps), dtype=np.uint16) if volumes else None
     ms = np.zeros(3, dtype=np.float64)
-    rc = lib().smvsb_sgm(int(device), w, h, _p(main_lum), nw, nh, _p(neigh_lum),
-                         _p(M), _p(t), C.c_float(min_depth), C.c_float(max_depth),
-                         int(num_steps), C.c_uint16(penalty1), C.c_uint16(penalty2),
-                         _p(depth), _p(cost), _p(S), _p(ms))
+    args = (int(device), w, h, _p(main_lum), nw, nh, _p(neigh_lum),
+            _p(M), _p(t), C.c_float(min_depth), C.c_float(max_depth),
+            int(num_steps), C.c_uint16(penalty1), C.c_uint16(penalty2),
+            _p(depth), _p(cost), _p(S), _p(ms))
+    if not device_bytes and not return_stats:
+        rc = lib().smvsb_sgm(*args)
+    else:
+        st, ex = _sgm_ex_args(device_bytes)
+        rc = lib().smvsb_sgm_ex(*args, *ex)
     if rc != 0:
         raise SmvsbError(rc, lib().smvsb_last_error(None).decode())
-    return dict(depth=depth, cost=cost, sgm=S, ms=ms)
+    out = dict(depth=depth, cost=cost, sgm=S, ms=ms)
+    return (out, _sgm_stats(st)) if return_stats else out
 
 
 def sgm_reconstruct(main_lum, neigh_lum, M_mn, t_mn, M_nm, t_nm, range_main, range_neigh,
-                    num_steps=128, penalty1=6, penalty2=96, merge_with=None, device=0):
+                    num_steps=128, penalty1=6, penalty2=96, merge_with=None, device=0, *,
+                    device_bytes=0, return_stats=False):
     """SGMStereo::reconstruct for one luminance pair (smvsb_sgm_reconstruct):
-    both directions, consistency check and optional merge on the device."""
+    both directions, consistency check and optional merge on the device.
+    device_bytes or return_stats select smvsb_sgm_reconstruct_ex, as in sgm()."""
     main_lum, neigh_lum = _u8(main_lum), _u8(neigh_lum)
     h, w = main_lum.shape
     nh, nw = neigh_lum.shape
@@ -457,12 +490,18 @@ def sgm_reconstruct(main_lum, neigh_lum, M_mn, t_mn, M_nm, t_nm, range_main, ran
     prev = _f32(merge_with)
     depth = np.empty((h, w), dtype=np.float32)
     ms = np.zeros(2, dtype=np.float64)
-    rc = lib().smvsb_sgm_reconstruct(
-        int(device), w, h, _p(main_lum), nw, nh, _p(neigh_lum), *[_p(a) for a in arrs],
-        int(num_steps), C.c_uint16(penalty1), C.c_uint16(penalty2), _p(prev), _p(depth), _p(ms))
+    args = (int(device), w, h, _p(main_lum), nw, nh, _p(neigh_lum), *[_p(a) for a in arrs],
+            int(num_steps), C.c_uint16(penalty1), C.c_uint16(penalty2), _p(prev), _p(depth),
+            _p(ms))
+    if not device_bytes and not return_stats:
+        rc = lib().smvsb_sgm_reconstruct(*args)
+    else:
+        st, ex = _sgm_ex_args(device_bytes)
+        rc = lib().smvsb_sgm_reconstruct_ex(*args, *ex)
     if rc != 0:
         raise SmvsbError(rc, lib().smvsb_last_error(None).decode())
-    return dict(depth=depth, ms=ms)
+    out = dict(depth=depth, ms=ms)
+    return (out, _sgm_stats(st)) if return_stats else out
 
 
 def measure_fp64_peak(device=0):

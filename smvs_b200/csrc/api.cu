@@ -1789,10 +1789,23 @@ smvsb_sgm (int device, int w, int h, const uint8_t* main_lum, int nw, int nh,
     uint16_t penalty2, float* depth_out, uint16_t* cost_out,
     uint16_t* sgm_out, double* ms_out)
 {
+    return smvsb_sgm_ex(device, w, h, main_lum, nw, nh, neigh_lum, M, t,
+        min_depth, max_depth, num_steps, penalty1, penalty2, depth_out,
+        cost_out, sgm_out, ms_out, nullptr, nullptr);
+}
+
+int
+smvsb_sgm_ex (int device, int w, int h, const uint8_t* main_lum, int nw,
+    int nh, const uint8_t* neigh_lum, const float* M, const float* t,
+    float min_depth, float max_depth, int num_steps, uint16_t penalty1,
+    uint16_t penalty2, float* depth_out, uint16_t* cost_out,
+    uint16_t* sgm_out, double* ms_out, const smvsb_sgm_options* opts,
+    smvsb_sgm_stats* stats)
+{
     return guarded(nullptr, [&]() {
         smvsb::sgm_run(device, w, h, main_lum, nw, nh, neigh_lum, M, t,
             min_depth, max_depth, num_steps, penalty1, penalty2, depth_out,
-            cost_out, sgm_out, ms_out);
+            cost_out, sgm_out, ms_out, opts, stats);
     });
 }
 
@@ -1804,10 +1817,26 @@ smvsb_sgm_reconstruct (int device, int w, int h, const uint8_t* main_lum,
     int num_steps, uint16_t penalty1, uint16_t penalty2,
     const float* merge_with, float* depth_out, double* ms_out)
 {
+    return smvsb_sgm_reconstruct_ex(device, w, h, main_lum, nw, nh,
+        neigh_lum, M_mn, t_mn, M_nm, t_nm, depth_range_main,
+        depth_range_neigh, num_steps, penalty1, penalty2, merge_with,
+        depth_out, ms_out, nullptr, nullptr);
+}
+
+int
+smvsb_sgm_reconstruct_ex (int device, int w, int h, const uint8_t* main_lum,
+    int nw, int nh, const uint8_t* neigh_lum, const float* M_mn,
+    const float* t_mn, const float* M_nm, const float* t_nm,
+    const float* depth_range_main, const float* depth_range_neigh,
+    int num_steps, uint16_t penalty1, uint16_t penalty2,
+    const float* merge_with, float* depth_out, double* ms_out,
+    const smvsb_sgm_options* opts, smvsb_sgm_stats* stats)
+{
     return guarded(nullptr, [&]() {
         smvsb::sgm_reconstruct(device, w, h, main_lum, nw, nh, neigh_lum,
             M_mn, t_mn, M_nm, t_nm, depth_range_main, depth_range_neigh,
-            num_steps, penalty1, penalty2, merge_with, depth_out, ms_out);
+            num_steps, penalty1, penalty2, merge_with, depth_out, ms_out,
+            opts, stats);
     });
 }
 

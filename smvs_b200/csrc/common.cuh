@@ -38,7 +38,7 @@ struct Error
     Error (int c, std::string const& m) : code(c), msg(m) {}
 };
 
-/* Owning device buffer; grows, never shrinks. */
+/* Owning device buffer; grows, and shrinks only by release(). */
 template <typename T>
 struct DevBuf
 {
@@ -65,6 +65,15 @@ struct DevBuf
         }
         cap = n;
     }
+
+    void release (void)
+    {
+        if (p) cudaFree(p);
+        p = nullptr;
+        cap = 0;
+    }
+
+    size_t bytes (void) const { return cap * sizeof(T); }
 };
 
 /* One neighbour view on the device: packed texels
@@ -251,6 +260,22 @@ check_device (int device)
         throw Error(SMVSB_ERR_INVALID, "device index out of range");
 }
 
+/* Free memory of the current device less a margin left to the runtime and
+ * the process's other work (1/32 of the card, at least 256 MiB): the start of
+ * the default budget of the calls that size their work to the device.
+ * total_out (may be NULL): the card's memory. */
+inline size_t
+usable_device_bytes (size_t* total_out = nullptr)
+{
+    size_t free_b = 0, total_b = 0;
+    CUDA_CHECK(cudaMemGetInfo(&free_b, &total_b));
+    if (total_out != nullptr)
+        *total_out = total_b;
+    size_t const margin = (total_b / 32 > (size_t(256) << 20))
+        ? total_b / 32 : (size_t(256) << 20);
+    return free_b > margin ? free_b - margin : 0;
+}
+
 inline SurfaceDev
 surface_args (smvsb_ctx* c)
 {
@@ -346,13 +371,15 @@ void sgm_run (int device, int w, int h, uint8_t const* main_lum, int nw, int nh,
     uint8_t const* neigh_lum, float const* M, float const* t,
     float min_depth, float max_depth, int num_steps, uint16_t penalty1,
     uint16_t penalty2, float* depth_out, uint16_t* cost_out,
-    uint16_t* sgm_out, double* ms_out);
+    uint16_t* sgm_out, double* ms_out, smvsb_sgm_options const* opts,
+    smvsb_sgm_stats* stats);
 void sgm_reconstruct (int device, int w, int h, uint8_t const* main_lum,
     int nw, int nh, uint8_t const* neigh_lum, float const* M_mn,
     float const* t_mn, float const* M_nm, float const* t_nm,
     float const* depth_range_main, float const* depth_range_neigh,
     int num_steps, uint16_t penalty1, uint16_t penalty2,
-    float const* merge_with, float* depth_out, double* ms_out);
+    float const* merge_with, float* depth_out, double* ms_out,
+    smvsb_sgm_options const* opts, smvsb_sgm_stats* stats);
 void cut_depth_maps_multi (smvsb_cut_options const* opts, int n_views,
     int const* w, int const* h, float const* const* depth,
     float const* const* normals, float const* invproj9,

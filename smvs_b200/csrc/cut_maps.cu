@@ -992,11 +992,7 @@ cut_depth_maps_multi (smvsb_cut_options const* opts, int n_views,
         if (dev_bytes == 0)
         {
             CUDA_CHECK(cudaSetDevice(d));
-            size_t free_b = 0, total_b = 0;
-            CUDA_CHECK(cudaMemGetInfo(&free_b, &total_b));
-            size_t const margin = std::max<size_t>(size_t(256) << 20,
-                total_b / 32);
-            dev_bytes = free_b > margin ? free_b - margin : 0;
+            dev_bytes = usable_device_bytes();
         }
         budget[k] = dev_bytes / share;
         if (budget[k] < least)

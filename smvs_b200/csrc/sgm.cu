@@ -22,6 +22,10 @@
  *       G = D / 16 lanes per pixel; S is only materialised when the caller
  *       asks for the volume.
  *
+ * When the volumes of a run do not fit the device budget (smvsb_sgm_ex), the
+ * same kernels run on bands of image rows in two sweeps with the paths' state
+ * carried across bands (run_banded); the depth is the same, bitwise.
+ *
  * Layouts: cost C[pixel][disp] uint8, sum S[pixel][disp] uint16 (pixel-major,
  * disparity contiguous, like the reference's sse_*_volume), so a warp's
  * access to one pixel is one coalesced 128 B / 256 B segment.
@@ -144,8 +148,9 @@ u8_to_float_kernel (size_t n, uint8_t const* __restrict__ in,
 
 /*
  * Warped neighbour volume: W[plane][row][col] = the byte
- * warped_neighbors_for_depth (:150-190) gives main pixel (col - 4, row - 3)
- * at that plane, 0 outside the image -- a margin of the census window's halo
+ * warped_neighbors_for_depth (:150-190) gives main pixel
+ * (col - 4, row0 + row - 3) at that plane, 0 outside the image (row0 > 0: a
+ * band of rows, see run_banded) -- a margin of the census window's halo
  * (4 columns, 3 rows, rounded up to the cost kernel's tiles) is part of the
  * volume, so the cost kernel loads its tiles without bounds tests. One thread
  * warps four neighbouring pixels through all planes (M * (x, y, 1) stays in
@@ -158,7 +163,7 @@ constexpr int WV_BX = 32, WV_BY = 4;
 __global__ void __launch_bounds__(WV_BX * WV_BY)
 sgm_warp_volume_kernel (SgmParams const p, float const* __restrict__ neigh,
     float const* __restrict__ depths, uint8_t* __restrict__ Wv, int pitch,
-    int rows)
+    int rows, int row0)
 {
     __shared__ float s_depths[256];
     int const tid = threadIdx.y * WV_BX + threadIdx.x;
@@ -169,7 +174,7 @@ sgm_warp_volume_kernel (SgmParams const p, float const* __restrict__ neigh,
     int const row = blockIdx.y * WV_BY + threadIdx.y;
     if (col >= pitch || row >= rows)
         return;
-    int const gy = row - 3;
+    int const gy = row0 + row - 3;
     float const nw1 = static_cast<float>(p.nw - 1);
     float const nh1 = static_cast<float>(p.nh - 1);
     float tp[4][3];
@@ -263,7 +268,7 @@ constexpr int C2_LOADS = (C2_LOAD_WORDS + C2_THREADS - 1) / C2_THREADS; /* 7 */
 
 __global__ void __launch_bounds__(C2_THREADS, 2)
 sgm_cost_bits_kernel (SgmParams const p, uint8_t const* __restrict__ main_img,
-    uint8_t const* __restrict__ Wv, int pitch, int rows,
+    uint8_t const* __restrict__ Wv, int pitch, int rows, int row0,
     uint8_t* __restrict__ cost)
 {
     /* [buffer][0 = pairs at even, 1 = at odd columns][plane][row][word],
@@ -277,6 +282,9 @@ sgm_cost_bits_kernel (SgmParams const p, uint8_t const* __restrict__ main_img,
     int const tx = tid % (C2_W / 4), ty = tid / (C2_W / 4);
     int const x0 = blockIdx.x * C2_W, y0 = blockIdx.y * C2_H;
     int const px = x0 + 4 * tx, py = y0 + ty;      /* first of four pixels */
+    /* y0, py: rows of the volume and of `cost`, which start at image row
+     * row0; gpy: the image row */
+    int const gpy = row0 + py;
 
     /* main image tile (0x6400 | byte, like the warped tiles), both copies */
     {
@@ -287,7 +295,7 @@ sgm_cost_bits_kernel (SgmParams const p, uint8_t const* __restrict__ main_img,
         for (int i = tid; i < C2_HALO_W * C2_HALO_H; i += C2_THREADS)
         {
             int const c = i % C2_HALO_W, r = i / C2_HALO_W;
-            int const gx = x0 - 4 + c, gy = y0 - 3 + r;
+            int const gx = x0 - 4 + c, gy = row0 + y0 - 3 + r;
             bool const in = (gx >= 0 && gx < p.w && gy >= 0 && gy < p.h);
             unsigned short const v = static_cast<unsigned short>(0x6400u
                 | (in ? main_img[gy * p.w + gx] : 0));
@@ -301,9 +309,9 @@ sgm_cost_bits_kernel (SgmParams const p, uint8_t const* __restrict__ main_img,
 #pragma unroll
     for (int i = 0; i < 4; ++i)
     {
-        in_px[i] = (px + i < p.w && py < p.h);
-        int_px[i] = in_px[i] && px + i >= 4 && px + i < p.w - 5 && py >= 3
-            && py < p.h - 4;
+        in_px[i] = (px + i < p.w && gpy < p.h);
+        int_px[i] = in_px[i] && px + i >= 4 && px + i < p.w - 5 && gpy >= 3
+            && gpy < p.h - 4;
     }
     __half2 const bias = as_half2(0x64006400u);          /* 1024.0 */
     /* census bits of the main pixels per window row (with the 0x6400 bias);
@@ -506,31 +514,52 @@ ilog2 (int n)
  * steps; a diagonal restarts at different steps on each, hence no branch
  * around the shuffles: the recurrence is always evaluated and a restarting
  * line overrides it.
+ *
+ * BANDED: one band of image rows [band.y0, band.y0 + band.rows) of a
+ * top-to-bottom sweep (band.sweep 0: L2R, R2L, T2B, T2B_D1, T2B_D2) or a
+ * bottom-to-top one (band.sweep 1: B2T, B2T_D1, B2T_D2); `cost` and `Dvol`
+ * hold the band's rows only. A vertical or diagonal line advances exactly one
+ * image row per step (the diagonals' wrap-around included), so a band is a
+ * range of its steps: the line's position after the steps of the bands before
+ * follows from its start, and its lanes' Pa..Pd are saved to band.state at the
+ * end of a band and reloaded at the start of the next.
  */
-template <int L>
+struct PathBand
+{
+    int y0, rows, sweep;
+    uint4* state;      /* [vertical direction][column][lane]: Pa, Pb, Pc, Pd */
+};
+
+template <int L, bool BANDED>
 __global__ void __launch_bounds__(128)
 sgm_paths_kernel (int w, int h, unsigned P1, unsigned P2,
-    uint8_t const* __restrict__ cost, uint8_t* __restrict__ Dvol)
+    uint8_t const* __restrict__ cost, uint8_t* __restrict__ Dvol,
+    PathBand const band)
 {
     constexpr int D = 8 * L;
     constexpr int LPW = 32 / L;                 /* lines per warp */
     int const grp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     int const lane = threadIdx.x & 31;
     int const sl = lane & (L - 1);              /* lane within the line */
-    int const hp = (h + LPW - 1) / LPW, wp = (w + LPW - 1) / LPW;
+    bool const up_sweep = BANDED && band.sweep != 0;
+    int const rows = BANDED ? band.rows : h;    /* rows of cost and Dvol */
+    int const n_horiz = up_sweep ? 0 : 2;       /* kinds of each group */
+    int const n_vert = BANDED ? 3 : 6;
+    int const first_vert = up_sweep ? PATH_B2T : PATH_T2B;
+    int const hp = (rows + LPW - 1) / LPW, wp = (w + LPW - 1) / LPW;
     int kind, line, count;
-    if (grp < 2 * hp)
+    if (grp < n_horiz * hp)
     {
         kind = grp / hp;                        /* PATH_L2R, PATH_R2L */
         line = LPW * (grp % hp) + (lane >> ilog2(L));
-        count = h;
+        count = rows;
     }
     else
     {
-        int const q = grp - 2 * hp;
-        if (q >= 6 * wp)
+        int const q = grp - n_horiz * hp;
+        if (q >= n_vert * wp)
             return;
-        kind = 2 + q / wp;                      /* PATH_T2B .. PATH_B2T_D2 */
+        kind = first_vert + q / wp;             /* PATH_T2B .. PATH_B2T_D2 */
         line = LPW * (q % wp) + (lane >> ilog2(L));
         count = w;
     }
@@ -541,9 +570,10 @@ sgm_paths_kernel (int w, int h, unsigned P1, unsigned P2,
     if (!live)
         line = count - 1;
     bool const horizontal = (kind < 2);
-    int const steps = horizontal ? w : h;
-    size_t const nvox = static_cast<size_t>(w) * h * D;
-    uint8_t* __restrict__ Dr = Dvol + static_cast<size_t>(kind) * nvox;
+    int const steps = horizontal ? w : rows;
+    size_t const nvox = static_cast<size_t>(w) * rows * D;
+    uint8_t* __restrict__ Dr = Dvol + static_cast<size_t>(kind
+        - (up_sweep ? PATH_B2T : 0)) * nvox;
 
     int x, y, dx, dy;
     switch (kind)
@@ -553,9 +583,9 @@ sgm_paths_kernel (int w, int h, unsigned P1, unsigned P2,
     case PATH_T2B: x = line; y = 0; dx = 0; dy = 1; break;
     case PATH_T2B_D1: x = line; y = 0; dx = 1; dy = 1; break;
     case PATH_T2B_D2: x = line; y = 0; dx = -1; dy = 1; break;
-    case PATH_B2T: x = line; y = h - 1; dx = 0; dy = -1; break;
-    case PATH_B2T_D1: x = line; y = h - 1; dx = 1; dy = -1; break;
-    default: x = line; y = h - 1; dx = -1; dy = -1; break;   /* B2T_D2 */
+    case PATH_B2T: x = line; y = rows - 1; dx = 0; dy = -1; break;
+    case PATH_B2T_D1: x = line; y = rows - 1; dx = 1; dy = -1; break;
+    default: x = line; y = rows - 1; dx = -1; dy = -1; break;   /* B2T_D2 */
     }
     int const restart_x = (dx > 0) ? 0 : w - 1;   /* diagonals only */
     bool const diagonal = (!horizontal && dx != 0);
@@ -563,12 +593,27 @@ sgm_paths_kernel (int w, int h, unsigned P1, unsigned P2,
     unsigned const P1x2 = P1 | (P1 << 16), P2x2 = P2 | (P2 << 16);
     unsigned const BIG = 0x7000u;          /* "no neighbour" sentinel */
     unsigned Pa = 0, Pb = 0, Pc = 0, Pd = 0;
+    bool start = true;
+    uint4* saved = nullptr;
+    if (BANDED && !horizontal)
+    {
+        /* steps this line took in the sweep's earlier bands */
+        int const done = (dy > 0) ? band.y0 : h - band.y0 - rows;
+        x = ((line + dx * (done % w)) % w + w) % w;
+        saved = band.state + (static_cast<size_t>(kind - PATH_T2B) * w
+            + line) * L + sl;
+        if (done > 0)
+        {
+            start = diagonal && x == restart_x;
+            uint4 const v = *saved;
+            Pa = v.x; Pb = v.y; Pc = v.z; Pd = v.w;
+        }
+    }
     long long const row_bytes = static_cast<long long>(w) * D;
     long long const step_bytes = dy * row_bytes + dx * D;
     uint8_t const* pc = cost + (static_cast<size_t>(y) * w + x) * D + sl * 8;
     uint8_t* pd = Dr + (static_cast<size_t>(y) * w + x) * D + sl * 8;
     uint2 c8 = *reinterpret_cast<uint2 const*>(pc);
-    bool start = true;
     for (int s = 0; s < steps; ++s)
     {
         int xn = x + dx;
@@ -621,6 +666,8 @@ sgm_paths_kernel (int w, int h, unsigned P1, unsigned P2,
         x = xn; pc += adv; pd += adv;
         start = diagonal && (xn == restart_x);
     }
+    if (BANDED && saved != nullptr && live)
+        *saved = make_uint4(Pa, Pb, Pc, Pd);
 }
 
 /*
@@ -637,6 +684,12 @@ sgm_paths_kernel (int w, int h, unsigned P1, unsigned P2,
  * fields), and the argmin -- lowest value, then lowest index, like the
  * reference's first minimum -- runs over the lane's 16 values and then over
  * the pixel's G lanes.
+ *
+ * The same kernel serves the banded path (rows [y0, y0 + rows) of the image;
+ * cost, Dvol, part_in and S_out hold those rows only): NV byte volumes,
+ * optionally a uint16 partial sum `part_in` in S's layout, and WTA = false
+ * writes the sum to S_out without the cost term or the winner. The current
+ * path is NV = 8, no partial sum, WTA, y0 = 0, rows = h.
  */
 __device__ __forceinline__ void
 wta_add16 (uint4 const v, unsigned mult, unsigned (&even)[4], unsigned (&odd)[4])
@@ -650,33 +703,50 @@ wta_add16 (uint4 const v, unsigned mult, unsigned (&even)[4], unsigned (&odd)[4]
     }
 }
 
-template <int G>
+template <int G, int NV, bool PART, bool WTA>
 __global__ void __launch_bounds__(256)
-sgm_sum_wta_kernel (int w, int h, uint8_t const* __restrict__ cost,
-    uint8_t const* __restrict__ Dvol, uint8_t const* __restrict__ main_img,
+sgm_sum_wta_kernel (int w, int h, int y0, int rows,
+    uint8_t const* __restrict__ cost, uint8_t const* __restrict__ Dvol,
+    uint16_t const* __restrict__ part_in, uint8_t const* __restrict__ main_img,
     float const* __restrict__ depths, uint16_t* __restrict__ S_out,
     float* __restrict__ out)
 {
     constexpr int D = 16 * G;
-    int const npix = w * h;
+    int const npix = w * rows;
     int const t = blockIdx.x * blockDim.x + threadIdx.x;
     int const p = t >> ilog2(G), sub = threadIdx.x & (G - 1);
     bool const on = p < npix;
     size_t const nvox = static_cast<size_t>(npix) * D;
     size_t const base = static_cast<size_t>(on ? p : 0) * D + sub * 16;
-    int const px = p % w, py = p / w;
+    int const px = p % w, py = y0 + p / w;
     unsigned const mult = 8u + (((px == 0 || px == w - 1)
         && (py == 0 || py == h - 1)) ? 1u : 0u);
     unsigned even[4] = { 0u, 0u, 0u, 0u }, odd[4] = { 0u, 0u, 0u, 0u };
-    uint4 v[9];
-    v[0] = __ldg(reinterpret_cast<uint4 const*>(cost + base));
+    uint4 v[NV + 1];
+    if (WTA)
+        v[0] = __ldg(reinterpret_cast<uint4 const*>(cost + base));
 #pragma unroll
-    for (int r = 0; r < 8; ++r)
+    for (int r = 0; r < NV; ++r)
         v[r + 1] = __ldg(reinterpret_cast<uint4 const*>(Dvol + r * nvox + base));
-    wta_add16(v[0], mult, even, odd);
+    if (WTA)
+        wta_add16(v[0], mult, even, odd);
 #pragma unroll
-    for (int r = 0; r < 8; ++r)
+    for (int r = 0; r < NV; ++r)
         wta_add16(v[r + 1], 1u, even, odd);
+    if (PART)
+    {
+        /* S's layout: word j of the 32 bytes = disparities (2j, 2j + 1) */
+        uint4 const* src = reinterpret_cast<uint4 const*>(part_in + base);
+        uint4 const lo = __ldg(src), hi = __ldg(src + 1);
+        unsigned const q[8] = { lo.x, lo.y, lo.z, lo.w, hi.x, hi.y, hi.z,
+            hi.w };
+#pragma unroll
+        for (int k = 0; k < 4; ++k)
+        {
+            even[k] += __byte_perm(q[2 * k], q[2 * k + 1], 0x5410);
+            odd[k] += __byte_perm(q[2 * k], q[2 * k + 1], 0x7632);
+        }
+    }
     if (S_out != nullptr && on)
     {
         /* disparities 4k .. 4k+3 of word k: even = (d0, d2), odd = (d1, d3) */
@@ -693,6 +763,8 @@ sgm_sum_wta_kernel (int w, int h, uint8_t const* __restrict__ cost,
         dst[0] = lo;
         dst[1] = hi;
     }
+    if (!WTA)
+        return;
     /* key = value << 16 | index; 0xffff is "no minimum found" (the reference
      * starts from numeric_limits<uint16_t>::max() and compares with <) */
     unsigned key = 0xffffffffu;
@@ -714,7 +786,8 @@ sgm_sum_wta_kernel (int w, int h, uint8_t const* __restrict__ cost,
     {
         int const idx = (key == 0xffffffffu) ? 0 : static_cast<int>(
             key & 0xffffu);
-        out[p] = (idx < 2 || main_img[p] < 25) ? 0.0f : depths[idx];
+        int const gp = y0 * w + p;
+        out[gp] = (idx < 2 || main_img[gp] < 25) ? 0.0f : depths[idx];
     }
 }
 
@@ -738,12 +811,12 @@ run_paths_wta (int w, int h, unsigned P1, unsigned P2, uint8_t const* cost,
     constexpr int L = D / 8, G = D / 16;        /* lanes per line / pixel */
     constexpr int LPW = 32 / L;                 /* lines per warp */
     int const warps = 2 * ((h + LPW - 1) / LPW) + 6 * ((w + LPW - 1) / LPW);
-    sgm_paths_kernel<L><<<(warps * 32 + 127) / 128, 128, 0, st>>>(w, h, P1,
-        P2, cost, Dvol);
+    sgm_paths_kernel<L, false><<<(warps * 32 + 127) / 128, 128, 0, st>>>(w,
+        h, P1, P2, cost, Dvol, PathBand{});
     CUDA_CHECK(cudaGetLastError());
     CUDA_CHECK(cudaEventRecord(mid, st));
-    sgm_sum_wta_kernel<G><<<(w * h * G + 255) / 256, 256, 0, st>>>(w, h,
-        cost, Dvol, main_img, depths, S_out, out);
+    sgm_sum_wta_kernel<G, 8, false, true><<<(w * h * G + 255) / 256, 256, 0,
+        st>>>(w, h, 0, h, cost, Dvol, nullptr, main_img, depths, S_out, out);
     CUDA_CHECK(cudaGetLastError());
 }
 
@@ -826,16 +899,21 @@ sgm_merge_kernel (size_t n, float const* __restrict__ first,
 }
 
 /* One workspace per device, shared by all host threads (calls on a device
- * serialise: the volumes of one 2 MP x 128 run take 2.4 GB). */
+ * serialise: the volumes of one 2 MP x 128 run take 2.4 GB). After a call it
+ * holds at most that call's budget (fit_workspace). */
 struct SgmWorkspace
 {
     std::mutex lock;
     bool ready = false;
     int device = 0;
+    size_t card_bytes = 0;
     cudaStream_t st = nullptr;
+    cudaStream_t copy = nullptr;     /* partial sums to and from the host */
     cudaEvent_t ev[8] = {};
+    cudaEvent_t band_ev[8] = {};     /* 4 per partial-sum slot, see run_banded */
     DevBuf<uint8_t> d_main, d_neigh, d_cost, d_D, d_warp;
-    DevBuf<uint16_t> d_S;
+    DevBuf<uint16_t> d_S, d_part;
+    DevBuf<uint4> d_state;
     DevBuf<float> d_depths, d_out, d_out2, d_prev, d_neigh_f;
 };
 
@@ -861,11 +939,9 @@ check_sgm_args (int w, int h, int nw, int nh, void const* a, void const* b,
 }
 
 /* The start of sgm_run and sgm_reconstruct: the workspace of `device`, held
- * by `hold` for the call, its stream ready and the two byte images on their
- * way to the device. */
+ * by `hold` for the call, with its streams ready. */
 SgmWorkspace&
-open_workspace (std::unique_lock<std::mutex>& hold, int device, int w, int h,
-    uint8_t const* main_lum, int nw, int nh, uint8_t const* neigh_lum)
+open_workspace (std::unique_lock<std::mutex>& hold, int device)
 {
     check_device(device);
     if (device >= SMVSB_MAX_DEVICES)
@@ -876,29 +952,440 @@ open_workspace (std::unique_lock<std::mutex>& hold, int device, int w, int h,
     if (!ws.ready)
     {
         CUDA_CHECK(cudaStreamCreateWithFlags(&ws.st, cudaStreamNonBlocking));
+        CUDA_CHECK(cudaStreamCreateWithFlags(&ws.copy,
+            cudaStreamNonBlocking));
         for (int i = 0; i < 8; ++i)
+        {
             CUDA_CHECK(cudaEventCreate(&ws.ev[i]));
+            CUDA_CHECK(cudaEventCreateWithFlags(&ws.band_ev[i],
+                cudaEventDisableTiming));
+        }
+        usable_device_bytes(&ws.card_bytes);
         ws.device = device;
         ws.ready = true;
     }
-    size_t const npix = static_cast<size_t>(w) * h;
-    size_t const nnpix = static_cast<size_t>(nw) * nh;
-    ws.d_main.reserve(npix);
-    ws.d_neigh.reserve(nnpix);
-    CUDA_CHECK(cudaMemcpyAsync(ws.d_main.p, main_lum, npix,
-        cudaMemcpyHostToDevice, ws.st));
-    CUDA_CHECK(cudaMemcpyAsync(ws.d_neigh.p, neigh_lum, nnpix,
-        cudaMemcpyHostToDevice, ws.st));
     return ws;
 }
 
-/* create_cost_volume + aggregate_sgm_costs + depth_from_sgm_volume for the
- * image pair already on the device; ev[e0 .. e0+3] bracket the three stages. */
+/* The two byte images on their way to the device. */
 void
-sgm_pair (SgmWorkspace& ws, int w, int h, uint8_t const* main_dev, int nw,
-    int nh, uint8_t const* neigh_dev, float const* M, float const* t,
-    float min_depth, float max_depth, int num_steps, unsigned P1, unsigned P2,
-    bool want_S, float* out_dev, int e0)
+upload_images (SgmWorkspace& ws, int w, int h, uint8_t const* main_lum,
+    int nw, int nh, uint8_t const* neigh_lum)
+{
+    CUDA_CHECK(cudaMemcpyAsync(ws.d_main.p, main_lum,
+        static_cast<size_t>(w) * h, cudaMemcpyHostToDevice, ws.st));
+    CUDA_CHECK(cudaMemcpyAsync(ws.d_neigh.p, neigh_lum,
+        static_cast<size_t>(nw) * nh, cudaMemcpyHostToDevice, ws.st));
+}
+
+/*
+ * What one run_sgm of a w x h image at D planes keeps on the device besides
+ * the images and depth maps, in elements of the workspace's buffers.
+ *  - The volume path: cost (1 B/voxel), eight L - C volumes (8 B) and the
+ *    warped volume with its margin (~1 B), for the whole image.
+ *  - The banded path, per band of band_rows rows: cost, five L - C volumes
+ *    (the most one sweep writes) and the warped volume with the census halo;
+ *    the uint16 partial sums, for the whole image on the device or two band
+ *    slots staged through the host; the carried state of the six vertical
+ *    directions (D / 8 uint4 per column).
+ */
+struct PairPlan
+{
+    bool banded = false, host_part = false;
+    int band_rows = 0, bands = 1;
+    size_t cost = 0, dvol = 0, warp = 0, S = 0, part = 0, state = 0;
+
+    size_t bytes (void) const
+    {
+        return cost + dvol + warp + (S + part) * sizeof(uint16_t)
+            + state * sizeof(uint4);
+    }
+};
+
+int
+warp_pitch (int w)
+{
+    return (w + C2_W - 1) / C2_W * C2_W + 16;
+}
+
+int
+warp_rows (int rows)
+{
+    return (rows + C2_H - 1) / C2_H * C2_H + 6;
+}
+
+PairPlan
+pair_plan (int w, int h, int D, int band_rows, bool host_part)
+{
+    PairPlan q;
+    q.banded = band_rows > 0;
+    q.host_part = q.banded && host_part;
+    int const r = q.banded ? band_rows : h;
+    q.band_rows = r;
+    q.bands = (h + r - 1) / r;
+    size_t const row_vox = static_cast<size_t>(w) * D;
+    q.cost = row_vox * r;
+    q.dvol = q.cost * (q.banded ? 5 : 8);
+    q.warp = static_cast<size_t>(warp_pitch(w)) * warp_rows(r) * D;
+    if (q.banded)
+    {
+        q.part = q.host_part ? 2 * q.cost : row_vox * h;
+        q.state = static_cast<size_t>(6) * w * (D / 8);
+    }
+    return q;
+}
+
+/* The bands on the banded path (they start at multiples of C2_H, so every
+ * band but the last fills whole cost tiles). Partial sums stay on the device
+ * when that still leaves bands of 64 rows or more (or as tall as host staging
+ * would give); band_rows 0: not even 16 rows fit `avail`. */
+PairPlan
+banded_plan (int w, int h, int D, size_t avail)
+{
+    auto most_rows = [&] (bool host) {
+        for (int r = (h + C2_H - 1) / C2_H * C2_H; r >= C2_H; r -= C2_H)
+            if (pair_plan(w, h, D, r, host).bytes() <= avail)
+                return r;
+        return 0;
+    };
+    int const on_device = most_rows(false), on_host = most_rows(true);
+    if (on_device > 0 && on_device >= std::min(on_host, 64))
+        return pair_plan(w, h, D, on_device, false);
+    PairPlan q = pair_plan(w, h, D, C2_H, true);
+    if (on_host > 0)
+        q = pair_plan(w, h, D, on_host, true);
+    else
+        q.band_rows = 0;
+    return q;
+}
+
+/* The volume path when it fits `avail` (or the dumps ask for the volumes),
+ * otherwise bands; throws when the budget does not hold one band. */
+PairPlan
+choose_plan (int w, int h, int D, bool dumps, size_t avail, size_t fixed,
+    size_t budget, bool default_budget)
+{
+    PairPlan q = pair_plan(w, h, D, 0, false);
+    if (dumps)
+        q.S = static_cast<size_t>(w) * h * D;
+    if (dumps || q.bytes() <= avail)
+        return q;
+    q = banded_plan(w, h, D, avail);
+    if (q.band_rows == 0)
+    {
+        /* the smaller of one 16-row band's needs with the partial sums on
+         * the device and with them staged (the device wins below 32 rows) */
+        size_t const least = fixed + std::min(
+            pair_plan(w, h, D, C2_H, false).bytes(),
+            pair_plan(w, h, D, C2_H, true).bytes());
+        throw Error(default_budget ? SMVSB_ERR_ALLOC : SMVSB_ERR_INVALID,
+            "smvsb_sgm: a device budget of " + std::to_string(budget)
+            + " bytes is below the minimum of " + std::to_string(least)
+            + " bytes for " + std::to_string(w) + "x"
+            + std::to_string(h) + " at " + std::to_string(D) + " planes "
+            "(one band of 16 rows and the carried state)");
+    }
+    return q;
+}
+
+/* The device bytes of the images, depths and depth maps a call keeps for
+ * its whole length. */
+struct Fixed
+{
+    size_t main = 0, neigh = 0, neigh_f = 0, out = 0, out2 = 0, prev = 0;
+
+    size_t bytes (void) const
+    {
+        return main + neigh + (neigh_f + out + out2 + prev + 512)
+            * sizeof(float);
+    }
+};
+
+/* fn(buffer, elements needed) over the buffers of the call's fixed data and
+ * over those of one run's volumes. */
+template <typename Fn>
+void
+each_fixed (SgmWorkspace& ws, Fixed const& f, Fn&& fn)
+{
+    fn(ws.d_main, f.main); fn(ws.d_neigh, f.neigh);
+    fn(ws.d_neigh_f, f.neigh_f); fn(ws.d_out, f.out);
+    fn(ws.d_out2, f.out2); fn(ws.d_prev, f.prev);
+    fn(ws.d_depths, size_t(512));
+}
+
+template <typename Fn>
+void
+each_volume (SgmWorkspace& ws, PairPlan const& q, Fn&& fn)
+{
+    fn(ws.d_cost, q.cost); fn(ws.d_D, q.dvol); fn(ws.d_warp, q.warp);
+    fn(ws.d_S, q.S); fn(ws.d_part, q.part); fn(ws.d_state, q.state);
+}
+
+/*
+ * Sizes the workspace for one run: the call's fixed buffers (fixed_live:
+ * already sized and holding data) and the run's volumes. When keeping every
+ * buffer at least as large as it is would exceed the budget -- or would not
+ * leave `later` bytes for a later run of the call -- the buffers larger than
+ * needed are released first, so the workspace never holds more than the
+ * budget (unless the volume dumps alone exceed it). Returns the bytes held.
+ */
+size_t
+fit_workspace (SgmWorkspace& ws, Fixed const& f, bool fixed_live,
+    PairPlan const& q, size_t budget, size_t later)
+{
+    size_t kept_fixed = 0, kept_vol = 0;
+    each_fixed(ws, f, [&] (auto& b, size_t n) {
+        kept_fixed += std::max(b.cap, n) * sizeof(*b.p); });
+    each_volume(ws, q, [&] (auto& b, size_t n) {
+        kept_vol += std::max(b.cap, n) * sizeof(*b.p); });
+    auto shrink = [] (auto& b, size_t n) { if (b.cap > n) b.release(); };
+    if (kept_fixed + std::max(kept_vol, later) > budget)
+    {
+        if (!fixed_live)
+            each_fixed(ws, f, shrink);
+        each_volume(ws, q, shrink);
+    }
+    size_t held = 0;
+    auto grow = [&] (auto& b, size_t n) {
+        b.reserve(n);
+        held += b.bytes();
+    };
+    each_fixed(ws, f, grow);
+    each_volume(ws, q, grow);
+    return held;
+}
+
+void
+release_workspace (SgmWorkspace& ws)
+{
+    auto drop = [] (auto& b, size_t) { b.release(); };
+    each_fixed(ws, Fixed{}, drop);
+    each_volume(ws, PairPlan{}, drop);
+}
+
+size_t
+held_bytes (SgmWorkspace& ws)
+{
+    size_t held = 0;
+    auto add = [&] (auto& b, size_t) { held += b.bytes(); };
+    each_fixed(ws, Fixed{}, add);
+    each_volume(ws, PairPlan{}, add);
+    return held;
+}
+
+void
+check_sgm_options (smvsb_sgm_options const* opts)
+{
+    if (opts != nullptr && (opts->reserved[0] != 0 || opts->reserved[1] != 0
+        || opts->reserved[2] != 0))
+        throw Error(SMVSB_ERR_INVALID,
+            "smvsb_sgm_options: reserved fields must be 0");
+}
+
+/* True when the run's buffers are larger than what the workspace holds. */
+bool
+grows (SgmWorkspace& ws, Fixed const& f, PairPlan const& q)
+{
+    bool more = false;
+    auto check = [&] (auto& b, size_t n) { more = more || n > b.cap; };
+    each_fixed(ws, f, check);
+    each_volume(ws, q, check);
+    return more;
+}
+
+/*
+ * The call's budget and the plans of its runs (plan(budget) returns them):
+ * opts->device_bytes, or the smaller of a quarter of the card and what is
+ * free (counting the workspace, which can be released) less the margin. The
+ * free memory is only asked for (a slow runtime query) when the plans within
+ * a quarter of the card need more than the workspace holds.
+ */
+template <typename Plan, typename Grows>
+size_t
+sgm_budget (SgmWorkspace& ws, smvsb_sgm_options const* opts, Plan&& plan,
+    Grows&& needs_more)
+{
+    if (opts != nullptr && opts->device_bytes != 0)
+    {
+        plan(opts->device_bytes);
+        return opts->device_bytes;
+    }
+    size_t budget = ws.card_bytes / 4;
+    plan(budget);
+    if (needs_more())
+    {
+        budget = std::min(budget, usable_device_bytes() + held_bytes(ws));
+        plan(budget);
+    }
+    return budget;
+}
+
+/* Pinned host memory for the partial sums of one call. */
+struct PinnedPart
+{
+    uint16_t* p = nullptr;
+    size_t cap = 0;
+
+    ~PinnedPart (void) { if (p) cudaFreeHost(p); }
+
+    void reserve (size_t n)
+    {
+        if (n <= cap)
+            return;
+        if (p) { cudaFreeHost(p); p = nullptr; cap = 0; }
+        cudaError_t const e = cudaHostAlloc(&p, n * sizeof(uint16_t),
+            cudaHostAllocDefault);
+        if (e != cudaSuccess)
+        {
+            p = nullptr;
+            throw Error(SMVSB_ERR_ALLOC, std::string("cudaHostAlloc of ")
+                + std::to_string(n * sizeof(uint16_t)) + " bytes: "
+                + cudaGetErrorString(e));
+        }
+        cap = n;
+    }
+};
+
+/* Warped volume and census cost of image rows [y0, y0 + rows) into d_cost
+ * (the whole image: y0 = 0, rows = h). */
+void
+launch_cost (SgmWorkspace& ws, SgmParams const& p, uint8_t const* main_dev,
+    float const* depths_dev, int y0, int rows)
+{
+    cudaStream_t st = ws.st;
+    /* warped volume with the cost tiles' halo as margin (zeros, written by
+     * the kernel itself) */
+    int const pitch = warp_pitch(p.w);
+    int const vrows = warp_rows(rows);
+    dim3 const wb(WV_BX, WV_BY);
+    dim3 const wg((pitch / 4 + WV_BX - 1) / WV_BX, (vrows + WV_BY - 1) / WV_BY);
+    sgm_warp_volume_kernel<<<wg, wb, 0, st>>>(p, ws.d_neigh_f.p, depths_dev,
+        ws.d_warp.p, pitch, vrows, y0);
+    CUDA_CHECK(cudaGetLastError());
+    dim3 const cg((p.w + C2_W - 1) / C2_W, (rows + C2_H - 1) / C2_H);
+    size_t const tile_bytes = sizeof(unsigned) * 2 * 2 * PLANES
+        * C2_HALO_H * C2_ROW_WORDS;
+    CUDA_CHECK(cudaFuncSetAttribute(sgm_cost_bits_kernel,
+        cudaFuncAttributeMaxDynamicSharedMemorySize,
+        static_cast<int>(tile_bytes)));
+    sgm_cost_bits_kernel<<<cg, C2_THREADS, tile_bytes, st>>>(p, main_dev,
+        ws.d_warp.p, pitch, vrows, y0, ws.d_cost.p);
+    CUDA_CHECK(cudaGetLastError());
+}
+
+/*
+ * run_sgm in bands of q.band_rows rows. Sweep 0, top to bottom: cost, the
+ * paths L2R, R2L, T2B, T2B_D1, T2B_D2 and their sum as uint16 partial sums
+ * (at most 5 * 255). Sweep 1, bottom to top: cost again, the paths B2T,
+ * B2T_D1, B2T_D2, and S = 8 C (+ the corner extra) + the three + the partial
+ * sum with the winner, as sgm_sum_wta_kernel does for the whole volume. The
+ * sums are integers: the depth is the volume path's.
+ * Host staging: band b's partial sums go through device slot b % 2. Sweep 0
+ * copies each slot to the host on the copy stream once it is written
+ * (band_ev[s]: written, [2 + s]: copied out); sweep 1 loads band b - 1 into
+ * its slot while band b runs (band_ev[4 + s]: loaded, [6 + s]: read). The
+ * last band's sums are still in their slot when sweep 1 starts.
+ * Returns the kernel launches.
+ */
+template <int D>
+int
+run_banded (SgmWorkspace& ws, SgmParams const& p, PairPlan const& q,
+    unsigned P1, unsigned P2, uint8_t const* main_dev, float const* depths_dev,
+    uint16_t* host_part, float* out_dev)
+{
+    constexpr int L = D / 8, G = D / 16;        /* lanes per line / pixel */
+    constexpr int LPW = 32 / L;                 /* lines per warp */
+    cudaStream_t st = ws.st, cp = ws.copy;
+    cudaEvent_t* const ev = ws.band_ev;
+    int const w = p.w, h = p.h, R = q.band_rows, nb = q.bands;
+    size_t const row_vox = static_cast<size_t>(w) * D;
+    size_t const band_vox = row_vox * R;
+    auto rows_of = [&] (int b) { return std::min(R, h - b * R); };
+    auto slot = [&] (int b) {
+        return ws.d_part.p + (q.host_part ? (b & 1) : b) * band_vox;
+    };
+    auto band_bytes = [&] (int b) {
+        return row_vox * rows_of(b) * sizeof(uint16_t);
+    };
+    int launches = 0;
+    for (int sweep = 0; sweep < 2; ++sweep)
+    {
+        for (int i = 0; i < nb; ++i)
+        {
+            int const b = (sweep == 0) ? i : nb - 1 - i;
+            int const y0 = b * R, rows = rows_of(b), s = b & 1;
+            if (sweep == 1 && q.host_part && b > 0)
+            {
+                /* load band b - 1 once band b + 1 has read its slot */
+                int const n = b - 1, sn = n & 1;
+                if (n + 2 <= nb - 1)
+                    CUDA_CHECK(cudaStreamWaitEvent(cp, ev[6 + sn], 0));
+                CUDA_CHECK(cudaMemcpyAsync(slot(n), host_part
+                    + static_cast<size_t>(n) * band_vox, band_bytes(n),
+                    cudaMemcpyHostToDevice, cp));
+                CUDA_CHECK(cudaEventRecord(ev[4 + sn], cp));
+            }
+            launch_cost(ws, p, main_dev, depths_dev, y0, rows);
+            int const n_horiz = (sweep == 0) ? 2 : 0;
+            int const warps = n_horiz * ((rows + LPW - 1) / LPW)
+                + 3 * ((w + LPW - 1) / LPW);
+            sgm_paths_kernel<L, true><<<(warps * 32 + 127) / 128, 128, 0,
+                st>>>(w, h, P1, P2, ws.d_cost.p, ws.d_D.p,
+                PathBand{ y0, rows, sweep, ws.d_state.p });
+            CUDA_CHECK(cudaGetLastError());
+            unsigned const blocks = static_cast<unsigned>(
+                (static_cast<size_t>(w) * rows * G + 255) / 256);
+            if (sweep == 0)
+            {
+                if (q.host_part && b >= 2)
+                    CUDA_CHECK(cudaStreamWaitEvent(st, ev[2 + s], 0));
+                sgm_sum_wta_kernel<G, 5, false, false><<<blocks, 256, 0,
+                    st>>>(w, h, y0, rows, nullptr, ws.d_D.p, nullptr,
+                    nullptr, nullptr, slot(b), nullptr);
+                CUDA_CHECK(cudaGetLastError());
+                if (q.host_part)
+                {
+                    CUDA_CHECK(cudaEventRecord(ev[s], st));
+                    CUDA_CHECK(cudaStreamWaitEvent(cp, ev[s], 0));
+                    CUDA_CHECK(cudaMemcpyAsync(host_part
+                        + static_cast<size_t>(b) * band_vox, slot(b),
+                        band_bytes(b), cudaMemcpyDeviceToHost, cp));
+                    CUDA_CHECK(cudaEventRecord(ev[2 + s], cp));
+                }
+            }
+            else
+            {
+                if (q.host_part && b < nb - 1)
+                    CUDA_CHECK(cudaStreamWaitEvent(st, ev[4 + s], 0));
+                sgm_sum_wta_kernel<G, 3, true, true><<<blocks, 256, 0,
+                    st>>>(w, h, y0, rows, ws.d_cost.p, ws.d_D.p, slot(b),
+                    main_dev, depths_dev, nullptr, out_dev);
+                CUDA_CHECK(cudaGetLastError());
+                if (q.host_part)
+                    CUDA_CHECK(cudaEventRecord(ev[6 + s], st));
+            }
+            launches += 4;
+        }
+    }
+    if (q.host_part)
+    {
+        /* nothing of the copy stream outlives the run */
+        CUDA_CHECK(cudaEventRecord(ev[0], cp));
+        CUDA_CHECK(cudaStreamWaitEvent(st, ev[0], 0));
+    }
+    return launches;
+}
+
+/* create_cost_volume + aggregate_sgm_costs + depth_from_sgm_volume for the
+ * image pair already on the device, in the workspace fit_workspace sized for
+ * plan q; ev[e0 .. e0+3] bracket the three stages (on the banded path they
+ * interleave: ev[e0 + 1] and ev[e0 + 2] are recorded at the end). */
+void
+sgm_pair (SgmWorkspace& ws, PairPlan const& q, int w, int h,
+    uint8_t const* main_dev, int nw, int nh, uint8_t const* neigh_dev,
+    float const* M, float const* t, float min_depth, float max_depth,
+    int num_steps, unsigned P1, unsigned P2, bool want_S, float* out_dev,
+    int e0, PinnedPart& pinned)
 {
     cudaStream_t st = ws.st;
     /* plane depths, lib/sgm_stereo.cc:195-203 (fp32 recurrence) */
@@ -913,15 +1400,8 @@ sgm_pair (SgmWorkspace& ws, int w, int h, uint8_t const* main_dev, int nw,
             inv_depth += increment;
         }
     }
-    size_t const npix = static_cast<size_t>(w) * h;
-    size_t const nvox = npix * num_steps;
-    ws.d_cost.reserve(nvox);
-    ws.d_D.reserve(nvox * 8);                 /* L - C per direction */
-    if (want_S)
-        ws.d_S.reserve(nvox);
     /* two slots: the first pair of a reconstruct call may still be reading
      * its depths when the second pair's are copied */
-    ws.d_depths.reserve(512);
     float* const depths_dev = ws.d_depths.p + (e0 != 0 ? 256 : 0);
     CUDA_CHECK(cudaMemcpyAsync(depths_dev, depths.data(),
         num_steps * sizeof(float), cudaMemcpyHostToDevice, st));
@@ -931,33 +1411,37 @@ sgm_pair (SgmWorkspace& ws, int w, int h, uint8_t const* main_dev, int nw,
     p.w = w; p.h = h; p.nw = nw; p.nh = nh; p.D = num_steps;
     std::copy(M, M + 9, p.M);
     std::copy(t, t + 3, p.t);
+    /* page-locking the host's partial sums takes the host a while: before
+     * the events, so that they time the device (a no-op in a reconstruct,
+     * which sizes the buffer for both runs) */
+    if (q.host_part)
+        pinned.reserve(static_cast<size_t>(w) * h * num_steps);
 
     CUDA_CHECK(cudaEventRecord(ws.ev[e0], st));
     /* float copy of the neighbour's byte image (part of the cost stage) */
     size_t const nnpix = static_cast<size_t>(nw) * nh;
-    ws.d_neigh_f.reserve(nnpix);
     u8_to_float_kernel<<<static_cast<unsigned>((nnpix + 255) / 256), 256, 0,
         st>>>(nnpix, neigh_dev, ws.d_neigh_f.p);
     CUDA_CHECK(cudaGetLastError());
-    /* warped volume with the cost tiles' halo as margin (zeros, written by
-     * the kernel itself) */
-    int const pitch = (w + C2_W - 1) / C2_W * C2_W + 16;
-    int const rows = (h + C2_H - 1) / C2_H * C2_H + 6;
-    ws.d_warp.reserve(static_cast<size_t>(pitch) * rows * num_steps);
-    dim3 const wb(WV_BX, WV_BY);
-    dim3 const wg((pitch / 4 + WV_BX - 1) / WV_BX, (rows + WV_BY - 1) / WV_BY);
-    sgm_warp_volume_kernel<<<wg, wb, 0, st>>>(p, ws.d_neigh_f.p, depths_dev,
-        ws.d_warp.p, pitch, rows);
-    CUDA_CHECK(cudaGetLastError());
-    dim3 const cg((w + C2_W - 1) / C2_W, (h + C2_H - 1) / C2_H);
-    size_t const tile_bytes = sizeof(unsigned) * 2 * 2 * PLANES
-        * C2_HALO_H * C2_ROW_WORDS;
-    CUDA_CHECK(cudaFuncSetAttribute(sgm_cost_bits_kernel,
-        cudaFuncAttributeMaxDynamicSharedMemorySize,
-        static_cast<int>(tile_bytes)));
-    sgm_cost_bits_kernel<<<cg, C2_THREADS, tile_bytes, st>>>(p, main_dev,
-        ws.d_warp.p, pitch, rows, ws.d_cost.p);
-    CUDA_CHECK(cudaGetLastError());
+
+    if (q.banded)
+    {
+        uint16_t* const host_part = q.host_part ? pinned.p : nullptr;
+        int launches = 0;
+        switch (num_steps)
+        {
+        case 32: launches = run_banded<32>(ws, p, q, P1, P2, main_dev, depths_dev, host_part, out_dev); break;
+        case 64: launches = run_banded<64>(ws, p, q, P1, P2, main_dev, depths_dev, host_part, out_dev); break;
+        case 128: launches = run_banded<128>(ws, p, q, P1, P2, main_dev, depths_dev, host_part, out_dev); break;
+        default: launches = run_banded<256>(ws, p, q, P1, P2, main_dev, depths_dev, host_part, out_dev); break;
+        }
+        count_device_launches(ws.device, 1 + launches);
+        for (int k = 1; k <= 3; ++k)
+            CUDA_CHECK(cudaEventRecord(ws.ev[e0 + k], st));
+        return;
+    }
+
+    launch_cost(ws, p, main_dev, depths_dev, 0, h);
     CUDA_CHECK(cudaEventRecord(ws.ev[e0 + 1], st));
 
     uint16_t* const S_dev = want_S ? ws.d_S.p : nullptr;
@@ -973,6 +1457,21 @@ sgm_pair (SgmWorkspace& ws, int w, int h, uint8_t const* main_dev, int nw,
     CUDA_CHECK(cudaEventRecord(ws.ev[e0 + 3], st));
 }
 
+void
+note_pair (smvsb_sgm_stats* stats, PairPlan const& q, size_t held, int w,
+    int h, int D)
+{
+    if (stats == nullptr)
+        return;
+    stats->banded |= q.banded ? 1 : 0;
+    stats->bands = std::max(stats->bands, q.bands);
+    stats->peak_device_bytes = std::max<uint64_t>(stats->peak_device_bytes,
+        held);
+    if (q.host_part)
+        stats->host_bytes += static_cast<uint64_t>(w) * h * D
+            * sizeof(uint16_t);
+}
+
 } /* namespace */
 
 void
@@ -980,22 +1479,36 @@ sgm_run (int device, int w, int h, uint8_t const* main_lum, int nw, int nh,
     uint8_t const* neigh_lum, float const* M, float const* t,
     float min_depth, float max_depth, int num_steps, uint16_t penalty1,
     uint16_t penalty2, float* depth_out, uint16_t* cost_out,
-    uint16_t* sgm_out, double* ms_out)
+    uint16_t* sgm_out, double* ms_out, smvsb_sgm_options const* opts,
+    smvsb_sgm_stats* stats)
 {
     check_sgm_args(w, h, nw, nh, main_lum, neigh_lum, M, t, depth_out,
         num_steps, penalty1, penalty2);
+    check_sgm_options(opts);
+    if (stats != nullptr)
+        *stats = smvsb_sgm_stats{};
     std::unique_lock<std::mutex> hold;
-    SgmWorkspace& ws = open_workspace(hold, device, w, h, main_lum, nw, nh,
-        neigh_lum);
+    SgmWorkspace& ws = open_workspace(hold, device);
     cudaStream_t st = ws.st;
     size_t const npix = static_cast<size_t>(w) * h;
     size_t const nvox = npix * num_steps;
-    ws.d_out.reserve(npix);
-    if (cost_out)
-        ws.d_S.reserve(nvox);
-    sgm_pair(ws, w, h, ws.d_main.p, nw, nh, ws.d_neigh.p, M, t, min_depth,
+    bool const dumps = (cost_out != nullptr || sgm_out != nullptr);
+    Fixed f;
+    f.main = npix; f.neigh = static_cast<size_t>(nw) * nh;
+    f.neigh_f = f.neigh; f.out = npix;
+    PairPlan q;
+    size_t const budget = sgm_budget(ws, opts, [&] (size_t b) {
+        size_t const avail = b > f.bytes() ? b - f.bytes() : 0;
+        q = choose_plan(w, h, num_steps, dumps, avail, f.bytes(), b,
+            opts == nullptr || opts->device_bytes == 0);
+    }, [&] { return grows(ws, f, q); });
+    size_t const held = fit_workspace(ws, f, false, q, budget, 0);
+    note_pair(stats, q, held, w, h, num_steps);
+    upload_images(ws, w, h, main_lum, nw, nh, neigh_lum);
+    PinnedPart pinned;
+    sgm_pair(ws, q, w, h, ws.d_main.p, nw, nh, ws.d_neigh.p, M, t, min_depth,
         max_depth, num_steps, penalty1, penalty2, sgm_out != nullptr,
-        ws.d_out.p, 0);
+        ws.d_out.p, 0, pinned);
     CUDA_CHECK(cudaMemcpyAsync(depth_out, ws.d_out.p, npix * sizeof(float),
         cudaMemcpyDeviceToHost, st));
     if (sgm_out)
@@ -1013,15 +1526,18 @@ sgm_run (int device, int w, int h, uint8_t const* main_lum, int nw, int nh,
             nvox * sizeof(uint16_t), cudaMemcpyDeviceToHost, st));
         CUDA_CHECK(cudaStreamSynchronize(st));
     }
+    /* the volume dumps are the one way past the budget: not kept */
+    if (held > budget)
+        release_workspace(ws);
+    float ms[3];
+    for (int i = 0; i < 3; ++i)
+        CUDA_CHECK(cudaEventElapsedTime(&ms[i], ws.ev[i], ws.ev[i + 1]));
     if (ms_out)
-    {
-        float ms;
         for (int i = 0; i < 3; ++i)
-        {
-            CUDA_CHECK(cudaEventElapsedTime(&ms, ws.ev[i], ws.ev[i + 1]));
-            ms_out[i] = ms;
-        }
-    }
+            ms_out[i] = q.banded ? (i == 0 ? ms[0] + ms[1] + ms[2] : 0.0)
+                : ms[i];
+    if (stats != nullptr)
+        stats->ms_device = ms[0] + ms[1] + ms[2];
 }
 
 /* SGMStereo::reconstruct (lib/sgm_stereo.cc:45-96) for an image pair at SGM
@@ -1033,33 +1549,55 @@ sgm_reconstruct (int device, int w, int h, uint8_t const* main_lum, int nw,
     float const* M_nm, float const* t_nm, float const* depth_range_main,
     float const* depth_range_neigh, int num_steps, uint16_t penalty1,
     uint16_t penalty2, float const* merge_with, float* depth_out,
-    double* ms_out)
+    double* ms_out, smvsb_sgm_options const* opts, smvsb_sgm_stats* stats)
 {
     check_sgm_args(w, h, nw, nh, main_lum, neigh_lum, M_mn, t_mn, depth_out,
         num_steps, penalty1, penalty2);
+    check_sgm_options(opts);
     if (!(nw > 9 && nh > 7 && M_nm && t_nm && depth_range_main
         && depth_range_neigh))
         throw Error(SMVSB_ERR_INVALID, "smvsb_sgm_reconstruct: bad arguments");
+    if (stats != nullptr)
+        *stats = smvsb_sgm_stats{};
     std::unique_lock<std::mutex> hold;
-    SgmWorkspace& ws = open_workspace(hold, device, w, h, main_lum, nw, nh,
-        neigh_lum);
+    SgmWorkspace& ws = open_workspace(hold, device);
     cudaStream_t st = ws.st;
     size_t const npix = static_cast<size_t>(w) * h;
-    ws.d_out.reserve(npix);
-    ws.d_out2.reserve(static_cast<size_t>(nw) * nh);
+    size_t const nnpix = static_cast<size_t>(nw) * nh;
+    bool const default_budget = opts == nullptr || opts->device_bytes == 0;
+    Fixed f;
+    f.main = npix; f.neigh = nnpix;
+    f.neigh_f = std::max(npix, nnpix);
+    f.out = npix; f.out2 = nnpix;
+    f.prev = (merge_with != nullptr) ? npix : 0;
+    /* sgm1: main against neighbour; sgm2: the roles swapped (:56-62) */
+    PairPlan q1, q2;
+    size_t const budget = sgm_budget(ws, opts, [&] (size_t b) {
+        size_t const avail = b > f.bytes() ? b - f.bytes() : 0;
+        q1 = choose_plan(w, h, num_steps, false, avail, f.bytes(), b,
+            default_budget);
+        q2 = choose_plan(nw, nh, num_steps, false, avail, f.bytes(), b,
+            default_budget);
+    }, [&] { return grows(ws, f, q1) || grows(ws, f, q2); });
+    size_t held = fit_workspace(ws, f, false, q1, budget, q2.bytes());
+    note_pair(stats, q1, held, w, h, num_steps);
+    upload_images(ws, w, h, main_lum, nw, nh, neigh_lum);
     if (merge_with != nullptr)
-    {
-        ws.d_prev.reserve(npix);
         CUDA_CHECK(cudaMemcpyAsync(ws.d_prev.p, merge_with,
             npix * sizeof(float), cudaMemcpyHostToDevice, st));
-    }
-    /* sgm1: main against neighbour; sgm2: the roles swapped (:56-62) */
-    sgm_pair(ws, w, h, ws.d_main.p, nw, nh, ws.d_neigh.p, M_mn, t_mn,
+    /* sized for both runs before the first: growing it between them would
+     * free memory the first run's copies may still use */
+    PinnedPart pinned;
+    pinned.reserve(std::max(q1.host_part ? npix * num_steps : 0,
+        q2.host_part ? nnpix * num_steps : 0));
+    sgm_pair(ws, q1, w, h, ws.d_main.p, nw, nh, ws.d_neigh.p, M_mn, t_mn,
         depth_range_main[0], depth_range_main[1], num_steps, penalty1,
-        penalty2, false, ws.d_out.p, 0);
-    sgm_pair(ws, nw, nh, ws.d_neigh.p, w, h, ws.d_main.p, M_nm, t_nm,
+        penalty2, false, ws.d_out.p, 0, pinned);
+    held = fit_workspace(ws, f, true, q2, budget, 0);
+    note_pair(stats, q2, held, nw, nh, num_steps);
+    sgm_pair(ws, q2, nw, nh, ws.d_neigh.p, w, h, ws.d_main.p, M_nm, t_nm,
         depth_range_neigh[0], depth_range_neigh[1], num_steps, penalty1,
-        penalty2, false, ws.d_out2.p, 4);
+        penalty2, false, ws.d_out2.p, 4, pinned);
 
     ConsistencyParams cp;
     cp.w = w; cp.h = h; cp.nw = nw; cp.nh = nh;
@@ -1082,14 +1620,16 @@ sgm_reconstruct (int device, int w, int h, uint8_t const* main_lum, int nw,
     CUDA_CHECK(cudaMemcpyAsync(depth_out, ws.d_out.p, npix * sizeof(float),
         cudaMemcpyDeviceToHost, st));
     CUDA_CHECK(cudaStreamSynchronize(st));
+    float ms[2];
+    CUDA_CHECK(cudaEventElapsedTime(&ms[0], ws.ev[0], ws.ev[3]));
+    CUDA_CHECK(cudaEventElapsedTime(&ms[1], ws.ev[4], ws.ev[7]));
     if (ms_out)
     {
-        float ms;
-        CUDA_CHECK(cudaEventElapsedTime(&ms, ws.ev[0], ws.ev[3]));
-        ms_out[0] = ms;
-        CUDA_CHECK(cudaEventElapsedTime(&ms, ws.ev[4], ws.ev[7]));
-        ms_out[1] = ms;
+        ms_out[0] = ms[0];
+        ms_out[1] = ms[1];
     }
+    if (stats != nullptr)
+        stats->ms_device = ms[0] + ms[1];
 }
 
 } /* namespace smvsb */
