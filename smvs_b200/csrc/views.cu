@@ -504,12 +504,21 @@ struct BilateralArgs
 };
 
 /* expf as glibc computes it (sysdeps/ieee754/flt-32/e_expf.c: N = 32 table,
- * cubic in double, one rounding to float), for -87 < x <= 0: the range weight
- * must be the bits the CPU produces. Checked against libm on 3e7 arguments
- * (tests/test_cpu_host.py runs the host twin of this function). */
+ * cubic in double, one rounding to float), for x <= 0: the range weight must
+ * be the bits the CPU produces. Checked against libm on 3e7 arguments in
+ * (-87, 0] and on [-1000, 0] (tests/test_cpu_host.py runs the host twin of
+ * this function). */
 __host__ __device__ __forceinline__ float
 expf_like_glibc (float x, unsigned long long const* tab)
 {
+    /* Below log(2^-150) glibc returns 0 (its underflow branch). The table
+     * path must not run there: below about x = -708 the exponent that
+     * ki << 47 adds to the table entry wraps past the smallest double
+     * exponent, and s turns into +-inf or a huge value. In the bilateral
+     * filter (argument -diff^2 / 0.02) two guide values more than 3.77 apart
+     * in one window would get an infinite or NaN weight instead of 0. */
+    if (x < -0x1.9fe368p6f)
+        return 0.0f;
     double const n = 32.0;
     double const c0 = 0x1.c6af84b912394p-5 / n / n / n;
     double const c1 = 0x1.ebfce50fac4f3p-3 / n / n;

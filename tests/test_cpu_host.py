@@ -234,6 +234,19 @@ def test_expf_twin_matches_libm():
                          np.float32([-0.0, -1e-7, -1.0, -50.0, -86.9])])
     for x in xs:
         assert L.smvsb_debug_expf(float(x)) == libm.expf(float(x))
+    # the whole of [-1000, 0]: the subnormal results of (-103.97, -87.3], the
+    # underflow bound log(2^-150) = -0x1.9fe368p6 and its neighbours, and the
+    # range below it where glibc returns 0 (a guide with values further apart
+    # than 3.77 in one window reaches it: the argument is -diff^2 / 0.02)
+    bound = np.float32(-float.fromhex("0x1.9fe368p6"))
+    xs = np.concatenate([-(rng.random(20000) * 1000).astype(np.float32),
+                         -(rng.random(5000) * 20 + 86).astype(np.float32),
+                         np.float32([-1000.0, -800.0, -720.0, -708.5, -200.0, -104.0,
+                                     -103.5, -87.5, -87.0]),
+                         [bound, np.nextafter(bound, np.float32(0)),
+                          np.nextafter(bound, np.float32(-np.inf))]])
+    for x in xs:
+        assert L.smvsb_debug_expf(float(x)) == libm.expf(float(x)), float(x)
 
 
 @pytest.mark.skipif(not oref.available(), reason="oracle/_ref not built")
